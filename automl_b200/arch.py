@@ -60,7 +60,7 @@ class DetArch(object):
     if p.data_format not in ('channels_last', 'channels_first'):
       raise ValueError('bad data_format %r' % (p.data_format,))
     if not p.separable_conv:
-      raise NotImplementedError('separable_conv=False is not on the B200 path')
+      raise NotImplementedError('separable_conv=False is not on the H100 path')
     if p.conv_bn_act_pattern or p.conv_after_downsample:
       raise NotImplementedError(
           'conv_bn_act_pattern / conv_after_downsample variants (SURVEY 8f.4)')

@@ -1,5 +1,5 @@
-"""Builds the in-tree CUDA library (sm_100a only) with nvcc.  No JIT cache: the .so lives next
-to the sources so it travels with the repo snapshot to the GPU box."""
+"""Builds the in-tree CUDA library (sm_90a only) with nvcc.  No JIT cache: the .so lives next
+to the sources, so the package imports from the source tree."""
 import hashlib
 import os
 import subprocess
@@ -10,7 +10,7 @@ LIB = os.path.join(CSRC, 'libautoml_b200.so')
 STAMP = LIB + '.stamp'
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
     '-Xcompiler', '-fPIC', '--shared',
 ]
 

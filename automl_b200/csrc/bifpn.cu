@@ -58,7 +58,7 @@ fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __res
           resample8(fi, base, c, y, x, ch, v);
           const float2 w2 = make_float2(fi.weight, fi.weight);
 #pragma unroll
-          for (int e = 0; e < 4; ++e) acc[e] = __ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), w2, acc[e]);
+          for (int e = 0; e < 4; ++e) acc[e] = ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), w2, acc[e]);
         }
       } else {
         // all raw loads first (same values, same accumulation order as the generic loop)
@@ -72,7 +72,7 @@ fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __res
         auto accumulate = [&](const float* v, float weight) {
           const float2 w2 = make_float2(weight, weight);
 #pragma unroll
-          for (int e = 0; e < 4; ++e) acc[e] = __ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), w2, acc[e]);
+          for (int e = 0; e < 4; ++e) acc[e] = ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), w2, acc[e]);
         };
         float v[8];
         resample_reduce<sig_mode(SIG, 0)>(raw0, taps0, v);
@@ -118,10 +118,10 @@ fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __res
           if (ky >= 0 && ky < 3) {
             const float4* wp = reinterpret_cast<const float4*>(wsm + (ky * 3 + kx) * kFuseCB + g * 8);
             const float4 w0 = wp[0], w1 = wp[1];
-            acc[r][0] = __ffma2_rn(make_float2(a.x, a.y), make_float2(w0.x, w0.y), acc[r][0]);
-            acc[r][1] = __ffma2_rn(make_float2(a.z, a.w), make_float2(w0.z, w0.w), acc[r][1]);
-            acc[r][2] = __ffma2_rn(make_float2(b.x, b.y), make_float2(w1.x, w1.y), acc[r][2]);
-            acc[r][3] = __ffma2_rn(make_float2(b.z, b.w), make_float2(w1.z, w1.w), acc[r][3]);
+            acc[r][0] = ffma2_rn(make_float2(a.x, a.y), make_float2(w0.x, w0.y), acc[r][0]);
+            acc[r][1] = ffma2_rn(make_float2(a.z, a.w), make_float2(w0.z, w0.w), acc[r][1]);
+            acc[r][2] = ffma2_rn(make_float2(b.x, b.y), make_float2(w1.x, w1.y), acc[r][2]);
+            acc[r][3] = ffma2_rn(make_float2(b.z, b.w), make_float2(w1.z, w1.w), acc[r][3]);
           }
         }
       }

@@ -25,9 +25,9 @@ static Option g_options[] = {
     {"dw_impl", 0, 2, {0}},          // 0 auto (tiled kernel where eligible), 1 register kernel only
     {"stem_impl", 0, 1, {0}},        // 0 tensor-core stem, 1 CUDA-core stem
     {"sepconv_impl", 0, 2, {0}},     // 0 TMA-staged input (1 buffer, 4 CTAs/SM), 1 loads from global, 2 TMA, 2 buffers, 3 CTAs/SM
-    {"pw_teams", 0, 3, {0}},         // 0 auto, 2 / 3 epilogue teams in pointwise_tc
-    {"pw_smem_kb", 0, 113, {0}},     // 0 auto, else shared-memory budget of a pointwise_tc CTA
-    {"persist_slack", 0, 148, {0}},  // CTAs a persistent kernel leaves out of its 2-per-SM grid
+    {"pw_teams", 0, 3, {0}},         // 0 auto, 2 / 3 consumer warpgroups in pointwise_tc
+    {"pw_smem_kb", 0, 227, {0}},     // 0 auto, else shared-memory budget of a pointwise_tc CTA
+    {"persist_slack", 0, 132, {0}},  // CTAs a persistent kernel leaves out of its grid
 };
 static Option* find_option(const char* name) {
   for (Option& o : g_options)
@@ -104,7 +104,7 @@ extern "C" int edet_set_option(const char* name, int value) {
                  o->lo, o->hi, value);
   EDET_CHECK_ARG(strcmp(name, "pw_teams") != 0 || value != 1, "set_option: pw_teams must be 0, 2 or 3");
   EDET_CHECK_ARG(strcmp(name, "pw_smem_kb") != 0 || value == 0 || value >= 64,
-                 "set_option: pw_smem_kb must be 0 or 64..113");
+                 "set_option: pw_smem_kb must be 0 or 64..227");
   o->value.store(value, std::memory_order_relaxed);
   return EDET_OK;
 }

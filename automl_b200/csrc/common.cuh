@@ -1,4 +1,4 @@
-// Shared device/host helpers for the automl_b200 kernels (sm_100a only).
+// Shared device/host helpers for the automl_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -69,19 +69,30 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   }
 }
 
-// Activation on a pair of values with the packed fp32 pipe of sm_100 (FADD2 / FMUL2 / FFMA2):
-// halves the ALU issue slots of the swish epilogues; the two MUFU ops per element remain.
+// Component-wise fp32 pair arithmetic, round to nearest.  sm_90 has no packed fp32 pipe, so each
+// is two scalar instructions; the results are those of the scalar ops.
+__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 fmul2_rn(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
+// Activation on a pair of values; the two MUFU ops per element dominate the swish epilogues.
 template <int ACT>
 __device__ __forceinline__ float2 apply_act2(float2 x) {
   if (ACT == EDET_ACT_SWISH) {
-    const float2 t = __fmul2_rn(x, make_float2(-1.4426950408889634f, -1.4426950408889634f));
+    const float2 t = fmul2_rn(x, make_float2(-1.4426950408889634f, -1.4426950408889634f));
     float2 e, r;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(t.x));
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(t.y));
-    const float2 d = __fadd2_rn(e, make_float2(1.f, 1.f));
+    const float2 d = fadd2_rn(e, make_float2(1.f, 1.f));
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.x) : "f"(d.x));   // rcp(inf) = 0: x -> -0 for x << 0
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.y) : "f"(d.y));
-    return __fmul2_rn(x, r);
+    return fmul2_rn(x, r);
   }
   return make_float2(apply_act_t<ACT>(x.x), apply_act_t<ACT>(x.y));
 }
@@ -99,20 +110,20 @@ __device__ __forceinline__ void apply_act4(float2& a, float2& b) {
     a.x = fmaxf(a.x, kLo); a.y = fmaxf(a.y, kLo);
     b.x = fmaxf(b.x, kLo); b.y = fmaxf(b.y, kLo);
     const float2 k = make_float2(-1.4426950408889634f, -1.4426950408889634f);
-    const float2 ta = __fmul2_rn(a, k), tb = __fmul2_rn(b, k);
+    const float2 ta = fmul2_rn(a, k), tb = fmul2_rn(b, k);
     float2 ea, eb;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ea.x) : "f"(ta.x));
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ea.y) : "f"(ta.y));
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(eb.x) : "f"(tb.x));
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(eb.y) : "f"(tb.y));
     const float2 one = make_float2(1.f, 1.f);
-    const float2 da = __fadd2_rn(ea, one), db = __fadd2_rn(eb, one);
-    const float2 p = __fmul2_rn(da, db);          // (d0*d2, d1*d3)
+    const float2 da = fadd2_rn(ea, one), db = fadd2_rn(eb, one);
+    const float2 p = fmul2_rn(da, db);          // (d0*d2, d1*d3)
     float r;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(p.x * p.y));
     const float2 q = make_float2(p.y * r, p.x * r);   // (1/(d0*d2), 1/(d1*d3))
-    a = __fmul2_rn(a, __fmul2_rn(db, q));             // x * 1/d0, x * 1/d1
-    b = __fmul2_rn(b, __fmul2_rn(da, q));
+    a = fmul2_rn(a, fmul2_rn(db, q));             // x * 1/d0, x * 1/d1
+    b = fmul2_rn(b, fmul2_rn(da, q));
     return;
   }
   a = apply_act2<ACT>(a);
@@ -198,7 +209,7 @@ inline int ensure_dynamic_smem(F kernel, int bytes, int* done) {
 // programmatic-stream-serialization attribute, signals `launch_dependents` as its first
 // instruction and executes `griddepcontrol.wait` before it touches global memory.  The NEXT
 // kernel's CTAs may therefore be scheduled, and run their prologue (smem carve-up, mbarrier
-// init, TMEM allocation, descriptor prefetch, weight preload into registers is NOT done before
+// init, descriptor prefetch, weight preload into registers is NOT done before
 // the wait), while the tail of the previous kernel drains -- the step is ~220 short launches.
 __device__ __forceinline__ void pdl_launch_dependents() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");

@@ -1,18 +1,19 @@
-// k x k convolution ('SAME', stride 1 or 2, NHWC fp16) as an implicit GEMM on the 5th-generation
-// tensor cores: the Fused-MBConv convolutions of EfficientNetV2
+// k x k convolution ('SAME', stride 1 or 2, NHWC fp16) as an implicit GEMM on the Hopper tensor
+// cores (wgmma): the Fused-MBConv convolutions of EfficientNetV2
 // (efficientnetv2/effnetv2_model.py:331-341 expand k x k + BN + act, :355-364 the single k x k conv
 // of expand_ratio == 1 blocks, :387-404 their use).
 //
 //   out[n, y, x, :] = act( sum_{ky,kx,c} in[n, y*s + ky - pt, x*s + kx - pl, c] * W[ky*k+kx][:, c] + bias )
 //                     (+ residual[n, y, x, :])
 //
-// Same persistent, warp-specialised structure as pointwise_tc.cu (TMA producer warp, MMA warp with
-// fp32 accumulators in TMEM, 8 epilogue warps with private TMA-store slabs, two CTAs per SM).
-// The M tile is an 8 x 16 block of output pixels; the K loop runs over (tap, 64-channel block):
-// for each tap the A operand is the SAME input tensor fetched by a 4-D TMA box {64 ch, 16, 8, 1}
-// shifted by the tap offset -- out-of-image pixels are zero-filled by TMA, which is exactly the
-// zero padding of 'SAME' -- so im2col never exists anywhere.  Stride 2 uses four tensor maps, one
-// per (row parity, column parity) sub-image of the input, so every tap is again a dense box.
+// Same persistent, warp-specialised structure as pointwise_tc.cu (TMA producer warp, two consumer
+// warpgroups taking tiles in turn, each with a stage ring of its own: wgmma main loop with fp32 accumulators in registers, then a
+// TMA-store epilogue, one CTA per SM).  The M tile is a 4 x 16 block of output pixels; the K loop
+// runs over (tap, 64-channel block): for each tap the A operand is the SAME input tensor fetched
+// by a 4-D TMA box {64 ch, 16, 4, 1} shifted by the tap offset -- out-of-image pixels are
+// zero-filled by TMA, which is exactly the zero padding of 'SAME' -- so im2col never exists
+// anywhere.  Stride 2 uses four tensor maps, one per (row parity, column parity) sub-image of the
+// input, so every tap is again a dense box.
 // Algorithmic HBM bytes per launch: 2*N*(H*W*Cin + Ho*Wo*Cout [+ residual]) + 2*k*k*Cout*Cin.
 #include "tc_common.cuh"
 
@@ -21,14 +22,17 @@ namespace convtc {
 
 using namespace pwtc;   // PTX wrappers and tensor-map encoders of tc_common.cuh
 
-constexpr int TH = 8, TW = 16;   // output pixel tile = the 128 rows of one UMMA
-
-
-constexpr int kThreads = 320;     // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue (two per TMEM lane quarter)
-constexpr int kEpiThreads = 256;
+constexpr int TH = 4, TW = 16;   // output pixel tile = the 64 rows of one wgmma
+constexpr int BLOCK_M = TH * TW;
+constexpr int kConsumers = 2;
+constexpr int kThreads = 128 * (1 + kConsumers);
+constexpr int kMaxBlockN = 128;
+constexpr int kNT = kMaxBlockN / 16;
 constexpr int kStoreCols = 64;
+constexpr int kSlabBytes = BLOCK_M * kStoreCols * 2;   // [64 px][64 cols] fp16, 128B swizzle
+constexpr int kSlabsPerTeam = kMaxBlockN / kStoreCols;
 constexpr int kMaxStages = 8;
-constexpr int kSmemLimit = 113 * 1024;                    // two CTAs per SM share the 227 KiB
+constexpr int kSmemLimit = 227 * 1024;                 // one CTA per SM
 
 struct Maps {
   CUtensorMap a[4];   // input (stride 1: a[0]) or its four (row parity, column parity) sub-images
@@ -40,13 +44,12 @@ struct Params {
   int batch, k, nout, nout_pad8;   // k = cin
   int ho, wo, ksize, stride, pad_t, pad_l, tiles_x, tiles_y, taps;
   int block_n, num_m_blocks, num_n_blocks, num_k_blocks, num_stages;
+  int team_stages;    // stages of each consumer's own ring: num_stages / kConsumers
   int block_k;        // 64 / 32 / 16 halves per k-block == 128B / 64B / 32B swizzled smem rows
   int a_stage_bytes, b_stage_bytes;
   int desc_sbo;       // byte distance between 8-row groups in smem (8 * row pitch)
-  int desc_layout;    // UMMA layout type: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
-  int slabs_per_warp; // private TMA-store staging slabs per epilogue warp (1 or 2)
-  int accum_stages;   // TMEM accumulator stages (2 when 2*block_n <= 256 columns, else 1)
-  int ldr, tmem_cols;
+  int desc_layout;    // wgmma layout type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
+  int ldr;
   int total_tiles;
   const float* bias;
   const __half* residual;
@@ -67,7 +70,7 @@ __device__ __forceinline__ TileCoord decode_tile(int t, const Params& p) {
 }
 
 template <int ACT, bool HAS_RES>
-__global__ void __launch_bounds__(kThreads, 2)
+__global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ Maps maps, const Params p) {
   const CUtensorMap& map_w = maps.w;
   const CUtensorMap& map_o = maps.o;
@@ -78,13 +81,9 @@ conv_tc_kernel(const __grid_constant__ Maps maps, const Params p) {
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
   uint8_t* smem_store = smem + p.num_stages * stage_bytes;
-  float* smem_bias = reinterpret_cast<float*>(smem_store + p.slabs_per_warp * (kEpiThreads / 32) * 4096);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_bias + 2 * 256);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_store + kConsumers * kSlabsPerTeam * kSlabBytes);
   uint64_t* full_bar = bars;                       // [kMaxStages]
   uint64_t* empty_bar = bars + kMaxStages;         // [kMaxStages]
-  uint64_t* tmem_full_bar = bars + 2 * kMaxStages;     // [2]
-  uint64_t* tmem_empty_bar = bars + 2 * kMaxStages + 2;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -92,41 +91,30 @@ conv_tc_kernel(const __grid_constant__ Maps maps, const Params p) {
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&tmem_full_bar[s]), 1);
-      mbar_init(smem_u32(&tmem_empty_bar[s]), kEpiThreads / 32);  // one arrive per epilogue warp
+      mbar_init(smem_u32(&empty_bar[s]), 4);       // one arrive per warp of the consumer
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.a[0])) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_o)) : "memory");
   }
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait_prior();          // everything above overlapped the previous kernel's tail
 
+  const int kk_per_tile = p.taps * p.num_k_blocks;
   if (warp == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      int stage_of[kConsumers] = {}, phase_of[kConsumers] = {};   // per consumer ring
       // bytes the two TMA boxes deliver (the B slot may be padded to 1 KiB)
       const uint32_t tx_bytes = static_cast<uint32_t>(p.a_stage_bytes + p.block_n * p.block_k * 2);
-      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+      int iter = 0;
+      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++iter) {
         const TileCoord tc = decode_tile(t, p);
-        for (int kk = 0; kk < p.taps * p.num_k_blocks; ++kk) {
+        const int team = iter % kConsumers;
+        int stage = stage_of[team];
+        uint32_t phase = static_cast<uint32_t>(phase_of[team]);
+        for (int kk = 0; kk < kk_per_tile; ++kk) {
           const int tap = kk / p.num_k_blocks, kb = kk - tap * p.num_k_blocks;
           const int ky = tap / p.ksize, kx = tap - ky * p.ksize;
           // input pixel of output (y, x) for this tap: (y*s + ry, x*s + rx)
@@ -138,195 +126,126 @@ conv_tc_kernel(const __grid_constant__ Maps maps, const Params p) {
             cy = tc.ty * TH + ((ry - py) >> 1);
             cx = tc.tx * TW + ((rx - px) >> 1);
           }
-          mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
-          const uint32_t fb = smem_u32(&full_bar[stage]);
+          const int s = team * p.team_stages + stage;
+          mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
+          const uint32_t fb = smem_u32(&full_bar[s]);
           mbar_expect_tx(fb, tx_bytes);
-          uint8_t* sa = smem + stage * stage_bytes;
+          uint8_t* sa = smem + s * stage_bytes;
           tma_load_4d(smem_u32(sa), &maps.a[map_id], fb, kb * p.block_k, cx, cy, tc.b);
           tma_load_3d(smem_u32(sa + p.a_stage_bytes), &map_w, fb, kb * p.block_k,
                       tc.n_blk * p.block_n, tap);
-          if (++stage == p.num_stages) {
+          if (++stage == p.team_stages) {
             stage = 0;
             phase ^= 1;
           }
         }
+        stage_of[team] = stage;
+        phase_of[team] = static_cast<int>(phase);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      // cute::UMMA::InstrDescriptor: c_format F32 (1<<4), a/b F16 (0), K-major both,
-      // n_dim = N>>3 at bit 17, m_dim = M>>4 at bit 24.
-      const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(p.block_n >> 3) << 17) |
-                             (static_cast<uint32_t>(BLOCK_M >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int iter = 0;
-      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++iter) {
-        const int as = p.accum_stages == 2 ? (iter & 1) : 0;
-        const uint32_t aphase = p.accum_stages == 2 ? ((iter >> 1) & 1) : (iter & 1);
-        mbar_wait(smem_u32(&tmem_empty_bar[as]), aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(as * p.block_n);
-        for (int kk = 0; kk < p.taps * p.num_k_blocks; ++kk) {
-          const int kb = kk % p.num_k_blocks;
-          mbar_wait(smem_u32(&full_bar[stage]), phase);
-          tc_fence_after();
-          uint8_t* sa = smem + stage * stage_bytes;
-          const uint64_t da = make_smem_desc(smem_u32(sa), p.desc_sbo, p.desc_layout);
-          const uint64_t db = make_smem_desc(smem_u32(sa + p.a_stage_bytes), p.desc_sbo, p.desc_layout);
-          const int k_rem = p.k - kb * p.block_k;
-          const int ksteps = k_rem >= p.block_k ? p.block_k / UMMA_K : (k_rem + UMMA_K - 1) / UMMA_K;
-          for (int ks = 0; ks < ksteps; ++ks) {
-            // advance 16 halves = 32 bytes inside the swizzle atom: +2 in the >>4 address field
-            tc_mma_f16(tmem_d, da + static_cast<uint64_t>(ks * 2), db + static_cast<uint64_t>(ks * 2),
-                       idesc, (kk > 0 || ks > 0) ? 1u : 0u);
-          }
-          tc_commit(smem_u32(&empty_bar[stage]));  // frees the smem stage when the MMAs retire
-          if (++stage == p.num_stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        tc_commit(smem_u32(&tmem_full_bar[as]));  // accumulator ready for the epilogue
-      }
-    }
-  } else {
-    // ===================== Epilogue (warps 2..9) =====================
-    // Fully decoupled warps: warp (quarter, team) owns rows quarter*32..+31 of the tile and the
-    // 64-column store chunks c == team (mod 2).  Each warp has a private 4 KiB staging slab and
-    // issues its own TMA stores ([32 rows x 64 cols] boxes), so the only synchronisation in the
-    // epilogue is the TMEM full/empty handshake with the MMA warp.
-    const int e_warp = warp - 2;              // 0..7
-    const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-    const int team = e_warp >> 2;             // even / odd store chunks
-    const int row_in_tile = quarter * 32 + lane;
-    uint8_t* my_slabs = smem_store + e_warp * p.slabs_per_warp * (32 * 128);
+  } else if (warp >= 4) {
+    // ===================== consumers: MMA + epilogue =====================
+    const int team = (warp >> 2) - 1;
+    const int wtid = threadIdx.x & 127;
+    const int r0 = 16 * (warp & 3) + (lane >> 2);   // tile rows (pixels) r0 and r0 + 8
+    const int cq = 2 * (lane & 3);
+    uint8_t* my_slabs = smem_store + team * kSlabsPerTeam * kSlabBytes;
+    const int b_chunk = p.block_k * 2;
+    int stage = 0;
+    uint32_t phase = 0;
     int iter = 0;
-    int store_cnt = 0;
     for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++iter) {
+      if (iter % kConsumers != team) continue;   // the other consumer's tile (and ring)
       const TileCoord tc = decode_tile(t, p);
-      const int as = p.accum_stages == 2 ? (iter & 1) : 0;
-      const uint32_t aphase = p.accum_stages == 2 ? ((iter >> 1) & 1) : (iter & 1);
       const int n0 = tc.n_blk * p.block_n;
-      const int oy = tc.ty * TH + row_in_tile / TW, ox = tc.tx * TW + row_in_tile % TW;
-      const bool row_ok = oy < p.ho && ox < p.wo;
-      const __half* res_row = nullptr;
-      if (HAS_RES) {
-        res_row = p.residual +
-                  ((static_cast<size_t>(tc.b) * p.ho + (row_ok ? oy : 0)) * p.wo + (row_ok ? ox : 0)) * p.ldr;
-      }
-      mbar_wait(smem_u32(&tmem_full_bar[as]), aphase);
-      tc_fence_after();
-      // only the columns that exist in the output are worth an epilogue (rounded up to the
-      // 16-column TMEM load granule); the rest of a ragged last N tile is skipped
       const int n_valid = min(p.block_n, ((p.nout - n0 + 15) >> 4) << 4);
-      const int num_chunks = (n_valid + kStoreCols - 1) / kStoreCols;
-      // last chunk this warp reads from TMEM (then the accumulator can be handed back)
-      int my_last = -1;
-      for (int c = team; c < num_chunks; c += 2) my_last = c;
-      if (my_last < 0) {
-        tc_fence_before();
+      const int nt = n_valid >> 4;
+      float acc[kNT][8];
+#pragma unroll
+      for (int j = 0; j < kNT; ++j)
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[j][q] = 0.f;
+      for (int kk = 0; kk < kk_per_tile; ++kk) {
+        const int kb = kk % p.num_k_blocks;
+        const int s = team * p.team_stages + stage;
+        mbar_wait(smem_u32(&full_bar[s]), phase);
+        uint8_t* sa = smem + s * stage_bytes;
+        const uint64_t da = make_smem_desc(smem_u32(sa), p.desc_sbo, p.desc_layout);
+        const uint64_t db = make_smem_desc(smem_u32(sa + p.a_stage_bytes), p.desc_sbo, p.desc_layout);
+        const int k_rem = p.k - kb * p.block_k;
+        const int ksteps = k_rem >= p.block_k ? p.block_k / MMA_K : (k_rem + MMA_K - 1) / MMA_K;
+        wg_fence();
+        wg_mma_kblock<kNT>(acc, da, db, b_chunk, nt, ksteps, kk == 0);
+        wg_commit();
+        wg_wait<0>();
         __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
+        if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));
+        if (++stage == p.team_stages) { stage = 0; phase ^= 1; }
       }
-      for (int c = team; c < num_chunks; c += 2) {
-        const int cols = min(kStoreCols, n_valid - c * kStoreCols);  // multiple of 16
-        uint8_t* my_stage = my_slabs + (p.slabs_per_warp == 2 ? (store_cnt & 1) * 4096 : 0);
-        ++store_cnt;
-        if (lane == 0) {                           // the store that last used this slab has left it
-          if (p.slabs_per_warp == 2) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
-        }
-        __syncwarp();
-        uint8_t* row_base = my_stage + lane * 128;
+      wg_fence_acc<kNT>(acc);
+      bool ok[2];
+      const __half* res_row[2] = {nullptr, nullptr};
 #pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          const int c_lo = hf * 32;
-          if (c_lo >= cols) break;
-          float v[32];
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) +
-                                 static_cast<uint32_t>(as * p.block_n + c * kStoreCols + c_lo);
+      for (int r = 0; r < 2; ++r) {
+        const int m = r0 + 8 * r;
+        const int oy = tc.ty * TH + m / TW, ox = tc.tx * TW + m % TW;
+        ok[r] = oy < p.ho && ox < p.wo;
+        if (HAS_RES)
+          res_row[r] = p.residual +
+                       ((static_cast<size_t>(tc.b) * p.ho + (ok[r] ? oy : 0)) * p.wo + (ok[r] ? ox : 0)) * p.ldr;
+      }
+      if (wtid == 0) tma_store_wait_read<0>();
+      named_sync(1 + team, 128);
 #pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            if (c_lo + g * 16 < cols) tc_ld16(taddr + g * 16, v + g * 16);
+      for (int j = 0; j < kNT; ++j) {
+        if (j < nt) {
+          const int colt = 16 * j + cq;
+          float b[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {     // columns colt, colt + 1, colt + 8, colt + 9
+            const int col = n0 + colt + (e >> 1) * 8 + (e & 1);
+            b[e] = col < p.nout ? __ldg(p.bias + col) : 0.f;
           }
-          tc_wait_ld();
-          if (c == my_last && (hf == 1 || c_lo + 32 >= cols)) {
-            // all TMEM reads of this warp for this accumulator are done
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
-          }
+          uint8_t* slab = my_slabs + (colt >> 6) * kSlabBytes;
+          const int piece = (colt & 63) >> 3;
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            if (c_lo + jj * 8 < cols) {
-              const int col = n0 + c * kStoreCols + c_lo + jj * 8;
-              float4 b0 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = b0;
-              if (col < p.nout_pad8) {          // a whole group of 8 biases is in bounds
-                b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-                b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col + 4));
-              } else if (col < p.nout) {        // ragged last group (nout % 8 != 0)
-                float bb[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) bb[e] = (col + e < p.nout) ? __ldg(p.bias + col + e) : 0.f;
-                b0 = make_float4(bb[0], bb[1], bb[2], bb[3]);
-                b1 = make_float4(bb[4], bb[5], bb[6], bb[7]);
-              }
-              float2 o2[4];
-              o2[0] = __fadd2_rn(make_float2(v[jj * 8 + 0], v[jj * 8 + 1]), make_float2(b0.x, b0.y));
-              o2[1] = __fadd2_rn(make_float2(v[jj * 8 + 2], v[jj * 8 + 3]), make_float2(b0.z, b0.w));
-              o2[2] = __fadd2_rn(make_float2(v[jj * 8 + 4], v[jj * 8 + 5]), make_float2(b1.x, b1.y));
-              o2[3] = __fadd2_rn(make_float2(v[jj * 8 + 6], v[jj * 8 + 7]), make_float2(b1.z, b1.w));
-              apply_act4<ACT>(o2[0], o2[1]);
-              apply_act4<ACT>(o2[2], o2[3]);
-              float o[8] = {o2[0].x, o2[0].y, o2[1].x, o2[1].y, o2[2].x, o2[2].y, o2[3].x, o2[3].y};
-              if (HAS_RES) {
-                if (row_ok && col < p.nout) {
-                  float r[8];
-                  half8_to_float(ldg_nc_v4(res_row + col), r);
-#pragma unroll
-                  for (int e = 0; e < 8; ++e) o[e] += r[e];
-                }
-              }
-              const uint4 packed = float_to_half8(o);
-              const int chunk16 = hf * 4 + jj;   // 16-byte piece inside the 128-byte row
-              *reinterpret_cast<uint4*>(row_base + ((chunk16 ^ (lane & 7)) << 4)) = packed;
+          for (int r = 0; r < 2; ++r) {
+            float2 lo = fadd2_rn(make_float2(acc[j][2 * r], acc[j][2 * r + 1]), make_float2(b[0], b[1]));
+            float2 hi = fadd2_rn(make_float2(acc[j][4 + 2 * r], acc[j][4 + 2 * r + 1]), make_float2(b[2], b[3]));
+            apply_act4<ACT>(lo, hi);
+            if (HAS_RES && ok[r]) {
+              const int col = n0 + colt;
+              if (col < p.nout)
+                lo = fadd2_rn(lo, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col)));
+              if (col + 8 < p.nout)
+                hi = fadd2_rn(hi, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col + 8)));
             }
+            const int row = r0 + 8 * r;
+            uint8_t* rb = slab + row * 128 + cq * 2;
+            *reinterpret_cast<__half2*>(rb + ((piece ^ (row & 7)) << 4)) = __floats2half2_rn(lo.x, lo.y);
+            *reinterpret_cast<__half2*>(rb + (((piece + 1) ^ (row & 7)) << 4)) = __floats2half2_rn(hi.x, hi.y);
           }
         }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          // the warp's 32 rows are two tile rows of 16 pixels: one 4-D box {64, 16, 2, 1}
-          tma_store_4d(&map_o, smem_u32(my_stage), n0 + c * kStoreCols, tc.tx * TW,
-                       tc.ty * TH + quarter * 2, tc.b);
-          tma_store_commit();
-        }
+      }
+      fence_proxy_async_smem();
+      named_sync(1 + team, 128);
+      if (wtid == 0) {
+        // the 64 rows are four tile rows of 16 pixels: one 4-D box {64, 16, 4, 1} per 64 columns
+        for (int c = 0; c * kStoreCols < n_valid; ++c)
+          tma_store_4d(&map_o, smem_u32(my_slabs + c * kSlabBytes), n0 + c * kStoreCols, tc.tx * TW,
+                       tc.ty * TH, tc.b);
+        tma_store_commit();
       }
     }
-    if (lane == 0) tma_store_wait_all();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
+    if (wtid == 0) tma_store_wait_all();
   }
 }
 
-// N tile.  Two CTAs are resident per SM (<=113 KiB smem, <=256 TMEM columns each):
-//   nout <= 128 : one tile, two accumulator stages;
-//   nout <= 256 : one tile, ONE accumulator stage (the other CTA of the SM hides the gap) --
-//                 avoids re-reading A and a ragged second tile for N = 144 / 240;
-//   wider       : tiles of 128 columns; the A tile of the extra tiles comes from L2 and the
-//                 epilogue skips the columns past nout.
+// N tile: the whole width up to 128 columns, else tiles of 128 (a multiple of the 64-column
+// store box); the A tile of the extra tiles comes from L2.
 static int pick_block_n(int nout) {
-  if (nout <= 256) return ((nout + 15) / 16) * 16;
-  return 128;
+  if (nout <= kMaxBlockN) return ((nout + 15) / 16) * 16;
+  return kMaxBlockN;
 }
 
 template <int ACT, bool HAS_RES>
@@ -361,8 +280,7 @@ extern "C" int edet_conv2d(const edet_half* in, const edet_half* wt, const float
   p.num_m_blocks = p.tiles_x * p.tiles_y;
   p.num_n_blocks = ceil_div(cout, p.block_n);
   p.block_k = cin <= 16 ? 16 : (cin <= 32 ? 32 : 64);
-  if (p.block_k == 64 && 2 * (BLOCK_M + p.block_n) * 128 + 40 * 1024 > kSmemLimit) p.block_k = 32;
-  p.desc_layout = p.block_k == 64 ? 2 : (p.block_k == 32 ? 4 : 6);
+  p.desc_layout = desc_layout_for(p.block_k);
   p.desc_sbo = 8 * p.block_k * 2;
   p.num_k_blocks = ceil_div(cin, p.block_k);
   p.a_stage_bytes = BLOCK_M * p.block_k * 2;
@@ -370,18 +288,15 @@ extern "C" int edet_conv2d(const edet_half* in, const edet_half* wt, const float
   p.ldr = cout;
   p.bias = bias;
   p.residual = reinterpret_cast<const __half*>(residual);
-  p.accum_stages = (2 * p.block_n <= 256) ? 2 : 1;
-  int cols = 32;
-  while (cols < p.accum_stages * p.block_n) cols *= 2;
-  p.tmem_cols = cols;
   p.total_tiles = n * p.num_m_blocks * p.num_n_blocks;
   const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
-  p.slabs_per_warp = stage_bytes <= 16 * 1024 ? 2 : 1;
-  const int fixed = p.slabs_per_warp * (kEpiThreads / 32) * 4096 + 2 * 256 * 4 +
-                    (2 * kMaxStages + 4) * 8 + 16;
+  const int fixed = kConsumers * kSlabsPerTeam * kSlabBytes + 2 * kMaxStages * 8;
   int stages = (kSmemLimit - 1024 - fixed) / stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
-  EDET_CHECK_ARG(stages >= 2, "conv2d: block_n %d leaves <2 pipeline stages", p.block_n);
+  p.team_stages = stages / kConsumers;       // each consumer's own ring
+  EDET_CHECK_ARG(p.team_stages >= 2, "conv2d: block_n %d leaves <2 pipeline stages per consumer",
+                 p.block_n);
+  stages = p.team_stages * kConsumers;
   p.num_stages = stages;
   const int smem_bytes = 1024 + stages * stage_bytes + fixed;
 
@@ -407,11 +322,11 @@ extern "C" int edet_conv2d(const edet_half* in, const edet_half* wt, const float
   if ((rc = make_map(&maps.w, wt, cin, cout, p.taps, cin, static_cast<uint64_t>(cout) * cin,
                      p.block_n, p.block_k)))
     return rc;
-  if ((rc = make_map4(&maps.o, out, cout, p.wo, p.ho, n, 64, TW, 2))) return rc;
+  if ((rc = make_map4(&maps.o, out, cout, p.wo, p.ho, n, kStoreCols, TW, TH))) return rc;
 
   const int sm_count = device_sm_count();
   if (!sm_count) return EDET_ERR_CUDA;
-  const int grid = p.total_tiles < 2 * sm_count ? p.total_tiles : 2 * sm_count;
+  const int grid = p.total_tiles < sm_count ? p.total_tiles : sm_count;
   const bool has_res = residual != nullptr;
   cudaStream_t s = as_stream(stream);
 #define EDET_CONV_CASE(A)                                                \

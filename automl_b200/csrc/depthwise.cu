@@ -5,7 +5,7 @@
 //   2 * n * c * (h*w + ho*wo) + 2 * k*k*c      (the SE squeeze adds 8*n*c bytes of atomics).
 //
 // Mapping: see depthwise_kernel below (register tile of 1 channel pair x 4 columns x ROWS rows,
-// fp32 accumulation with packed FFMA2; coalesced 128-byte warp accesses along the channel axis).
+// fp32 accumulation with FFMA on channel pairs; coalesced 128-byte warp accesses along the channel axis).
 #include "common.cuh"
 
 namespace edet {
@@ -24,7 +24,7 @@ struct DwCfg {
 // Register tiling: one thread owns ONE channel pair (a half2, so a warp reads 128 contiguous
 // bytes of the NHWC row), kDwTW adjacent output columns and ROWS output rows.  Every loaded
 // input is converted to fp32 once and reused by up to K*K taps from registers; the arithmetic is
-// the packed fp32 FMA of sm_100 (FFMA2) on the channel pair.  Rationale: a 5x5 depthwise conv
+// fp32 FMAs on the channel pair.  Rationale: a 5x5 depthwise conv
 // needs 25 MACs per output element, more than the scalar FFMA pipe can issue at the HBM rate,
 // and without the column tiling the half->float conversions of the kx re-reads dominate.
 template <int K, int S, int ACT, bool HAS_BIAS, bool HAS_SE>
@@ -102,7 +102,7 @@ depthwise_kernel(const __half* __restrict__ in, __half* __restrict__ out,
             for (int tx = 0; tx < TW; ++tx)
 #pragma unroll
               for (int kx = 0; kx < K; ++kx)
-                acc[r][tx] = __ffma2_rn(xv[tx * S + kx], wreg[ky * K + kx], acc[r][tx]);
+                acc[r][tx] = ffma2_rn(xv[tx * S + kx], wreg[ky * K + kx], acc[r][tx]);
           }
         }
       }
@@ -131,7 +131,7 @@ depthwise_kernel(const __half* __restrict__ in, __half* __restrict__ out,
             for (int tx = 0; tx < TW; ++tx)
 #pragma unroll
               for (int kx = 0; kx < K; ++kx)
-                acc[r][tx] = __ffma2_rn(xv[tx * S + kx], wreg[ky * K + kx], acc[r][tx]);
+                acc[r][tx] = ffma2_rn(xv[tx * S + kx], wreg[ky * K + kx], acc[r][tx]);
           }
         }
       }
@@ -146,14 +146,14 @@ depthwise_kernel(const __half* __restrict__ in, __half* __restrict__ out,
       if (interior || oy0 + r < ho) {
         float2 o[TW];
 #pragma unroll
-        for (int tx = 0; tx < TW; ++tx) o[tx] = __fadd2_rn(acc[r][tx], bv);
+        for (int tx = 0; tx < TW; ++tx) o[tx] = fadd2_rn(acc[r][tx], bv);
 #pragma unroll
         for (int tx = 0; tx + 1 < TW; tx += 2) apply_act4<ACT>(o[tx], o[tx + 1]);
         if (TW & 1) o[TW - 1] = apply_act2<ACT>(o[TW - 1]);
 #pragma unroll
         for (int tx = 0; tx < TW; ++tx) {
           if (interior || ox0 + tx < wo) {
-            if (HAS_SE) ssum = __fadd2_rn(ssum, o[tx]);
+            if (HAS_SE) ssum = fadd2_rn(ssum, o[tx]);
             orow[tx * cp_count] = __floats2half2_rn(o[tx].x, o[tx].y);
           }
         }

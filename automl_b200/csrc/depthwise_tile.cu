@@ -7,7 +7,7 @@
 // border predicates and a single code path; a ring of NSTAGE tiles keeps the next work units in
 // flight while the current one is computed.  Compute: one lane = one channel pair (a warp reads
 // the 128 contiguous bytes of a pixel, conflict-free), one thread = TR x TC outputs of that pair
-// from registers (fp32 weights in registers, packed FFMA2), one warp = one TR x TC patch, the 8
+// from registers (fp32 weights in registers, FFMA on channel pairs), one warp = one TR x TC patch, the 8
 // warps of a CTA tile a (TR*WY) x (TC*WX) output tile.  HBM sees each input byte once per tile
 // (plus the halo, served by L2) and each output byte once.
 //
@@ -190,7 +190,7 @@ dw_tile_kernel(const __grid_constant__ CUtensorMap map_x, const Params p) {
           for (int tx = 0; tx < TC; ++tx)
 #pragma unroll
             for (int kx = 0; kx < K; ++kx)
-              acc[r][tx] = __ffma2_rn(xv[tx * S + kx], wreg[ky * K + kx], acc[r][tx]);
+              acc[r][tx] = ffma2_rn(xv[tx * S + kx], wreg[ky * K + kx], acc[r][tx]);
         }
       }
     }
@@ -206,14 +206,14 @@ dw_tile_kernel(const __grid_constant__ CUtensorMap map_x, const Params p) {
         if (oy0 + r < p.ho) {
           float2 o[TC];
 #pragma unroll
-          for (int tx = 0; tx < TC; ++tx) o[tx] = __fadd2_rn(acc[r][tx], bv);
+          for (int tx = 0; tx < TC; ++tx) o[tx] = fadd2_rn(acc[r][tx], bv);
 #pragma unroll
           for (int tx = 0; tx + 1 < TC; tx += 2) apply_act4<ACT>(o[tx], o[tx + 1]);
           if (TC & 1) o[TC - 1] = apply_act2<ACT>(o[TC - 1]);
 #pragma unroll
           for (int tx = 0; tx < TC; ++tx) {
             if (ox0 + tx < p.wo) {
-              if (HAS_SE) ssum = __fadd2_rn(ssum, o[tx]);
+              if (HAS_SE) ssum = fadd2_rn(ssum, o[tx]);
               orow[static_cast<size_t>(tx) * cp_total] = __floats2half2_rn(o[tx].x, o[tx].y);
             }
           }

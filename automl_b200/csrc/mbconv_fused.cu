@@ -8,16 +8,16 @@
 // "plan B").  Algorithmic HBM bytes per launch: 2*N*(H*W*Cin*halo + Ho*Wo*Cmid) + weights,
 // instead of 2*N*(H*W*Cin + 2*H*W*Cmid + Ho*Wo*Cmid) for the two separate kernels.
 //
-// One CTA works on a 16x16 INPUT patch (256 pixels = two 128-row MMA blocks) and one chunk of
-// the expanded channels:
+// One CTA works on a 16x16 INPUT patch (256 pixels = four 64-row wgmma blocks, two per warpgroup)
+// and one chunk of the expanded channels:
 //   1. TMA (4-D map over the NHWC input, out-of-image pixels zero-filled) -> smem A tile
 //      [256 px][Cin], TMA -> smem W tile [ch][Cin]   (32B / 64B / 128B swizzle by Cin)
-//   2. tcgen05.mma: E[256 px][ch] = A * W^T into TMEM (fp32)
-//   3. all 8 warps: tcgen05.ld -> +bias -> act -> fp16 -> smem E tile; pixels outside the image
-//      become 0 (TF pads the EXPANDED tensor with zeros, not the input)
+//   2. wgmma: E[256 px][ch] = A * W^T, fp32 accumulators in registers
+//   3. every thread: its accumulator fragment -> +bias -> act -> fp16 -> smem E tile; pixels
+//      outside the image become 0 (TF pads the EXPANDED tensor with zeros, not the input)
 //   4. all 8 warps: depthwise kxk stride s over the smem E tile (one channel pair x one output
-//      row per work item, packed FFMA2), + bias + act -> global, SE sums -> int64 atomics
-// The next tile's TMA loads are issued as soon as the MMA of the current tile has retired, so
+//      row per work item, FFMA on channel pairs), + bias + act -> global, SE sums -> int64 atomics
+// The next tile's TMA loads are issued as soon as the MMAs of the current tile have retired, so
 // they overlap steps 3-4.
 #include "tc_common.cuh"
 
@@ -29,7 +29,8 @@ using namespace pwtc;
 constexpr int kThreads = 256;
 constexpr int kPatch = 16;                 // input patch is kPatch x kPatch pixels
 constexpr int kPatchPx = kPatch * kPatch;  // 256 rows of the expand GEMM
-constexpr int kMaxCh = 128;                // expanded channels per tile (2 x 128 TMEM columns)
+constexpr int kMaxCh = 64;                 // expanded channels per tile: 2 x 32 accumulators per thread
+constexpr int kNT = kMaxCh / 16;
 // bytes per pixel row of the smem E tile: (pitch / 16) odd -> conflict-free 128-bit row writes;
 // a compile-time constant so that every depthwise tap is an immediate offset
 constexpr int kEPitch = kMaxCh * 2 + 16;
@@ -54,7 +55,6 @@ struct Params {
   int ch, num_chunks;          // expanded channels per CTA tile, number of chunks
   int oth, otw;                // output tile (rows, cols) produced from one input patch
   int tiles_y, tiles_x, total_tiles;
-  int tmem_cols;
   const float* bias_e;         // [cmid]
   const float* wd;             // fp32 depthwise taps [k*k][cmid]
   const float* bias_d;         // [cmid]
@@ -93,39 +93,24 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
   unsigned long long* se_s =
       reinterpret_cast<unsigned long long*>(smem_e + kPatchPx * kEPitch);  // [ch]
   uint64_t* bars = reinterpret_cast<uint64_t*>(se_s + p.ch);
-  const uint32_t full_bar = smem_u32(bars);       // TMA -> MMA            (thread 0 only)
-  const uint32_t kb_bar = smem_u32(bars + 1);     // MMA k-block retired   (thread 0 only)
-  const uint32_t acc_bar = smem_u32(bars + 2);    // accumulator complete  (everyone)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
-  volatile int* next_tile_s = reinterpret_cast<volatile int*>(tmem_slot + 1);
+  const uint32_t full_bar = smem_u32(bars);       // TMA -> MMA
+  volatile int* next_tile_s = reinterpret_cast<volatile int*>(bars + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;                       // warpgroup: patch pixels 128 wg .. 128 wg + 127
   if (threadIdx.x == 0) {
     mbar_init(full_bar, 1);
-    mbar_init(kb_bar, 1);
-    mbar_init(acc_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
   }
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait_prior();
 
   const uint32_t tx_bytes = static_cast<uint32_t>(kPatchPx * p.block_k * 2 + p.ch * p.block_k * 2);
-  const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(p.ch >> 3) << 17) |
-                         (static_cast<uint32_t>(BLOCK_M >> 4) << 24);
-  uint32_t full_phase = 0, kb_phase = 0, acc_phase = 0;
+  const int pitch = p.block_k * 2;                // bytes per smem operand row
+  const int nt = p.ch >> 4;
+  uint32_t full_phase = 0;
 
   auto issue_loads = [&](const Tile& tl, int kb) {
     mbar_expect_tx(full_bar, tx_bytes);
@@ -142,37 +127,28 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
     const Tile tl = decode(t, p);
     const int cbase = tl.chunk * p.ch;
     const int cv = min(p.ch, p.cmid - cbase);   // valid channels of this chunk (multiple of 8)
-    // ---- 1+2. expand GEMM into TMEM (thread 0 drives TMA and MMA) ----
-    if (threadIdx.x == 0) {
-      for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-        if (!(kb == 0 && prefetched)) issue_loads(tl, kb);
-        mbar_wait(full_bar, full_phase);
-        full_phase ^= 1;
-        tc_fence_after();
-        const int k_rem = p.cin - kb * p.block_k;
-        const int ksteps = k_rem >= p.block_k ? p.block_k / UMMA_K : (k_rem + UMMA_K - 1) / UMMA_K;
-        const uint64_t db = make_smem_desc(smem_u32(smem_b), p.desc_sbo, p.desc_layout);
-#pragma unroll 1
-        for (int mb = 0; mb < 2; ++mb) {
-          const uint64_t da =
-              make_smem_desc(smem_u32(smem_a + mb * (p.a_bytes >> 1)), p.desc_sbo, p.desc_layout);
-          for (int ks = 0; ks < ksteps; ++ks)
-            tc_mma_f16(tmem_base + static_cast<uint32_t>(mb * p.ch),
-                       da + static_cast<uint64_t>(ks * 2), db + static_cast<uint64_t>(ks * 2),
-                       idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-        }
-        if (kb + 1 < p.num_k_blocks) {   // the single operand buffer is reused by the next k-block
-          tc_commit(kb_bar);
-          mbar_wait(kb_bar, kb_phase);
-          kb_phase ^= 1;
-        } else {
-          tc_commit(acc_bar);
-        }
+    // ---- 1+2. expand GEMM (thread 0 drives TMA; each warpgroup multiplies its 128 pixels) ----
+    float acc[2][kNT][8] = {};
+    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+      if (threadIdx.x == 0 && !(kb == 0 && prefetched)) issue_loads(tl, kb);
+      mbar_wait(full_bar, full_phase);
+      full_phase ^= 1;
+      const int k_rem = p.cin - kb * p.block_k;
+      const int ksteps = k_rem >= p.block_k ? p.block_k / MMA_K : (k_rem + MMA_K - 1) / MMA_K;
+      const uint64_t db = make_smem_desc(smem_u32(smem_b), p.desc_sbo, p.desc_layout);
+      wg_fence();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint64_t da =
+            make_smem_desc(smem_u32(smem_a + (wg * 128 + h * 64) * pitch), p.desc_sbo, p.desc_layout);
+        wg_mma_kblock<kNT>(acc[h], da, db, pitch, nt, ksteps, kb == 0);
       }
+      wg_commit();
+      wg_wait<0>();
+      __syncthreads();   // every MMA of this k-block has retired: the operand buffers are free
     }
-    mbar_wait(acc_bar, acc_phase);
-    acc_phase ^= 1;
-    tc_fence_after();
+    wg_fence_acc<kNT>(acc[0]);
+    wg_fence_acc<kNT>(acc[1]);
     // the operand buffers are free: fetch the next tile's first k-block under phases 3-4
     if (threadIdx.x == 0) {
       const int tn = sched_next_tile(p.sched, p.total_tiles);
@@ -180,44 +156,45 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
       prefetched = tn < p.total_tiles;
       if (prefetched) issue_loads(decode(tn, p), 0);
     }
-    // ---- 3. TMEM -> bias, act, mask -> smem E tile ----
+    // ---- 3. accumulator fragments -> bias, act, mask -> smem E tile ----
     {
-      const int mb = warp >> 2, quarter = warp & 3;
-      const int m = mb * 128 + quarter * 32 + lane;        // patch pixel of this thread
-      const int py = m / kPatch, px = m % kPatch;
-      const int iy = tl.ty * OTW * S - p.pad_t + py, ix = tl.tx * OTW * S - p.pad_l + px;
-      const bool inside = iy >= 0 && iy < p.h && ix >= 0 && ix < p.w;
-      const uint32_t erow = smem_u32(smem_e) + m * kEPitch;
+      const int cq = 2 * (lane & 3);
       const float* be = p.bias_e + cbase;
-      for (int c0 = 0; c0 < cv; c0 += 16) {
-        float v[16];
-        tc_ld16(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) +
-                    static_cast<uint32_t>(mb * p.ch + c0), v);
-        tc_wait_ld();
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c0 + g * 8 < cv) {
-            uint4 packed = make_uint4(0u, 0u, 0u, 0u);   // TF zero-pads the EXPANDED map
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int m = wg * 128 + h * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * r;  // patch pixel
+          const int py = m / kPatch, px = m % kPatch;
+          const int iy = tl.ty * OTW * S - p.pad_t + py, ix = tl.tx * OTW * S - p.pad_l + px;
+          const bool inside = iy >= 0 && iy < p.h && ix >= 0 && ix < p.w;
+          const uint32_t erow = smem_u32(smem_e) + m * kEPitch;
+#pragma unroll
+          for (int j = 0; j < kNT; ++j) {
+            const int col = 16 * j + cq;
+            if (16 * j >= cv) continue;
+            const bool hi_ok = 16 * j + 8 < cv;     // cv is a multiple of 8
+            uint32_t lo_bits = 0u, hi_bits = 0u;    // TF zero-pads the EXPANDED map
             if (inside) {
-              const float4 b0 = __ldg(reinterpret_cast<const float4*>(be + c0 + g * 8));
-              const float4 b1 = __ldg(reinterpret_cast<const float4*>(be + c0 + g * 8 + 4));
-              float2 r0 = __fadd2_rn(make_float2(v[g * 8 + 0], v[g * 8 + 1]), make_float2(b0.x, b0.y));
-              float2 r1 = __fadd2_rn(make_float2(v[g * 8 + 2], v[g * 8 + 3]), make_float2(b0.z, b0.w));
-              float2 r2 = __fadd2_rn(make_float2(v[g * 8 + 4], v[g * 8 + 5]), make_float2(b1.x, b1.y));
-              float2 r3 = __fadd2_rn(make_float2(v[g * 8 + 6], v[g * 8 + 7]), make_float2(b1.z, b1.w));
-              apply_act4<ACT>(r0, r1);
-              apply_act4<ACT>(r2, r3);
-              const float o[8] = {r0.x, r0.y, r1.x, r1.y, r2.x, r2.y, r3.x, r3.y};
-              packed = float_to_half8(o);
+              const float2 b_lo = __ldg(reinterpret_cast<const float2*>(be + col));
+              const float2 b_hi = hi_ok ? __ldg(reinterpret_cast<const float2*>(be + col + 8))
+                                        : make_float2(0.f, 0.f);
+              float2 lo = fadd2_rn(make_float2(acc[h][j][2 * r], acc[h][j][2 * r + 1]), b_lo);
+              float2 hi = fadd2_rn(make_float2(acc[h][j][4 + 2 * r], acc[h][j][4 + 2 * r + 1]), b_hi);
+              apply_act4<ACT>(lo, hi);
+              const __half2 l2 = __floats2half2_rn(lo.x, lo.y), h2 = __floats2half2_rn(hi.x, hi.y);
+              lo_bits = *reinterpret_cast<const uint32_t*>(&l2);
+              hi_bits = *reinterpret_cast<const uint32_t*>(&h2);
             }
-            sts_v4(erow + (c0 + g * 8) * 2, packed);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(erow + col * 2), "r"(lo_bits) : "memory");
+            if (hi_ok)
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(erow + (col + 8) * 2), "r"(hi_bits) : "memory");
           }
         }
       }
       if (HAS_SE)
         for (int i = threadIdx.x; i < p.ch; i += kThreads) se_s[i] = 0ull;
     }
-    tc_fence_before();   // the TMEM reads are ordered before the next tile's MMA by this barrier
     __syncthreads();
     // ---- 4. depthwise over the smem E tile ------------------------------------------------------
     {
@@ -262,7 +239,7 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
                 for (int tx = 0; tx < CG; ++tx)
 #pragma unroll
                   for (int kx = 0; kx < K; ++kx)
-                    acc[r][tx] = __ffma2_rn(xv[tx * S + kx], wk[ky * K + kx], acc[r][tx]);
+                    acc[r][tx] = ffma2_rn(xv[tx * S + kx], wk[ky * K + kx], acc[r][tx]);
               }
             }
           }
@@ -273,15 +250,15 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
           float2 ssum = make_float2(0.f, 0.f);
 #pragma unroll
           for (int r = 0; r < OTW; ++r) {
-            float2 o0 = __fadd2_rn(acc[r][0], bd), o1 = __fadd2_rn(acc[r][1], bd);
+            float2 o0 = fadd2_rn(acc[r][0], bd), o1 = fadd2_rn(acc[r][1], bd);
             apply_act4<ACT>(o0, o1);
             if (r < rows) {
               if (xg * CG < cols) {
-                if (HAS_SE) ssum = __fadd2_rn(ssum, o0);
+                if (HAS_SE) ssum = fadd2_rn(ssum, o0);
                 ocol[static_cast<size_t>(r) * p.wo * cm2] = __floats2half2_rn(o0.x, o0.y);
               }
               if (xg * CG + 1 < cols) {
-                if (HAS_SE) ssum = __fadd2_rn(ssum, o1);
+                if (HAS_SE) ssum = fadd2_rn(ssum, o1);
                 ocol[static_cast<size_t>(r) * p.wo * cm2 + cm2] = __floats2half2_rn(o1.x, o1.y);
               }
             }
@@ -311,7 +288,7 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
 #pragma unroll
             for (int kx = 0; kx < K; ++kx) {
               if ((ixl - kx) >= 0 && (ixl - kx) % S == 0 && (ixl - kx) / S < OTW)
-                acc[(ixl - kx) / S] = __ffma2_rn(v, wk[kx], acc[(ixl - kx) / S]);
+                acc[(ixl - kx) / S] = ffma2_rn(v, wk[kx], acc[(ixl - kx) / S]);
             }
           }
         }
@@ -320,7 +297,7 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
                         ((static_cast<size_t>(tl.n) * p.ho + oy0 + oyl) * p.wo + ox0) * cm2 +
                         (cbase >> 1) + cp;
 #pragma unroll
-        for (int i = 0; i < OTW; ++i) acc[i] = __fadd2_rn(acc[i], bd);
+        for (int i = 0; i < OTW; ++i) acc[i] = fadd2_rn(acc[i], bd);
 #pragma unroll
         for (int i = 0; i + 1 < OTW; i += 2) apply_act4<ACT>(acc[i], acc[i + 1]);
         if (OTW & 1) acc[OTW - 1] = apply_act2<ACT>(acc[OTW - 1]);
@@ -328,7 +305,7 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
 #pragma unroll
         for (int oxl = 0; oxl < OTW; ++oxl) {
           if (oxl < cols) {
-            if (HAS_SE) ssum = __fadd2_rn(ssum, acc[oxl]);
+            if (HAS_SE) ssum = fadd2_rn(ssum, acc[oxl]);
             orow[static_cast<size_t>(oxl) * cm2] = __floats2half2_rn(acc[oxl].x, acc[oxl].y);
           }
         }
@@ -347,18 +324,7 @@ mbconv_front_kernel(const __grid_constant__ CUtensorMap map_x,
       }
     }
     __syncthreads();   // E tile (and se_s) free for the next tile; next_tile_s published
-    tc_fence_after();
     t = next_tile_s[it & 1];
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
   }
 }
 
@@ -399,17 +365,14 @@ extern "C" int edet_mbconv_expand_dw(const edet_half* x, const edet_half* we, co
   p.n = n; p.h = h; p.w = w; p.cin = cin; p.cmid = cmid;
   p.ho = ceil_div(h, stride); p.wo = ceil_div(w, stride);
   p.pad_t = same_pad_before(h, k, stride); p.pad_l = same_pad_before(w, k, stride);
-  // channel chunks: <= 128 accumulator columns per 128-row block, so that two CTAs (2 x 2 x 128
-  // TMEM columns) share an SM; the last chunk may be partial (weights beyond cmid are TMA
-  // zero-fill and never read back)
-  p.num_chunks = ceil_div(cmid, 128);
+  // channel chunks: <= kMaxCh accumulator columns (2 x kMaxCh / 2 registers per thread), so that
+  // two CTAs share an SM; the last chunk may be partial (weights beyond cmid are TMA zero-fill and
+  // never read back)
+  p.num_chunks = ceil_div(cmid, kMaxCh);
   p.ch = ((ceil_div(cmid, p.num_chunks) + 15) / 16) * 16;
   p.oth = p.otw = (kPatch - k) / stride + 1;
   p.tiles_y = ceil_div(p.ho, p.oth); p.tiles_x = ceil_div(p.wo, p.otw);
   p.total_tiles = n * p.tiles_y * p.tiles_x * p.num_chunks;
-  int cols = 32;
-  while (cols < 2 * p.ch) cols *= 2;
-  p.tmem_cols = cols;
   int smem_bytes = 0;
   for (int bk = cin <= 16 ? 16 : (cin <= 32 ? 32 : 64); bk >= 16; bk >>= 1) {
     p.block_k = bk;
@@ -419,7 +382,7 @@ extern "C" int edet_mbconv_expand_dw(const edet_half* x, const edet_half* we, co
     if (smem_bytes <= 113 * 1024 || bk == 32) break;   // two CTAs per SM, else settle for 32
   }
   p.num_k_blocks = ceil_div(cin, p.block_k);
-  p.desc_layout = p.block_k == 64 ? 2 : (p.block_k == 32 ? 4 : 6);
+  p.desc_layout = desc_layout_for(p.block_k);
   p.desc_sbo = 8 * p.block_k * 2;
   p.bias_e = bias_e; p.bias_d = bias_d;
   p.wd = wd;
@@ -435,9 +398,8 @@ extern "C" int edet_mbconv_expand_dw(const edet_half* x, const edet_half* we, co
     return rc;
   const int sm_count = device_sm_count();
   if (!sm_count) return EDET_ERR_CUDA;
-  // CTAs per SM the resources allow (smem and TMEM columns)
+  // CTAs per SM the shared memory allows
   int per_sm = 232448 / (smem_bytes + 1024);
-  if (per_sm * p.tmem_cols > 512) per_sm = 512 / p.tmem_cols;
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 2) per_sm = 2;
   const int grid = p.total_tiles < per_sm * sm_count ? p.total_tiles : per_sm * sm_count;

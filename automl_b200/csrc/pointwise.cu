@@ -1,4 +1,4 @@
-// edet_pointwise_conv: argument checks + dispatch (tcgen05 path / SIMT cross-check kernel).
+// edet_pointwise_conv: argument checks + dispatch (wgmma path / SIMT cross-check kernel).
 #include "tc_common.cuh"
 
 namespace edet {

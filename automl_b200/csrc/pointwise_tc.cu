@@ -1,20 +1,20 @@
-// Pointwise (1x1) convolution as an NHWC GEMM on the 5th-generation tensor cores (sm_100a).
+// Pointwise (1x1) convolution as an NHWC GEMM on the Hopper tensor cores (wgmma, sm_90a).
 //
 //   out[b, r, n] = act( sum_k A[b, r, k] * Wt[b|0, n, k] + bias[n] ) (+ residual[b, r, n])
 //
-// Structure (persistent CTAs, two per SM so one CTA's epilogue overlaps the other's loads;
-// 192 threads each):
-//   warp 0      : TMA producer  -- cp.async.bulk.tensor (3-D maps, 128B swizzle) for the A tile
-//                 [128 x 64] and the W tile [block_n x 64] into an N-stage smem ring (mbarrier
-//                 complete_tx).  Out-of-bounds rows / K tail are zero-filled by TMA.
-//   warp 1      : allocates TMEM, then one lane issues tcgen05.mma (kind::f16, M=128,
-//                 N=block_n, K=16) with fp32 accumulators in TMEM, double-buffered across tiles;
-//                 tcgen05.commit releases smem stages / publishes the accumulator.
-//   warps 2..9  : epilogue -- tcgen05.ld (32x32b) -> +bias -> activation -> (+residual) -> fp16 ->
-//                 swizzled st.shared -> TMA store (cp.async.bulk.tensor ... bulk_group), which
-//                 also clips the ragged M / N edges.  Two warps share each TMEM lane quarter and
-//                 split every 64-column store chunk into two 32-column halves (the swish
-//                 epilogue is MUFU / issue bound, so it gets 8 warps and packed fp32 math).
+// Structure (persistent CTAs, one per SM, warp-specialised):
+//   warpgroup 0        : warp 0 / lane 0 is the TMA producer -- cp.async.bulk.tensor (3-D maps,
+//                        128B / 64B / 32B swizzle) of the A tile [64 x block_k] and the W tile
+//                        [block_n x block_k] into the smem stage ring of the consumer that owns
+//                        the tile (mbarrier complete_tx).  Each consumer has a ring of its own, so
+//                        it sees every phase of its stage barriers (a consumer that skipped the
+//                        other's stages could meet a barrier two phases behind, whose parity looks
+//                        complete).  Out-of-bounds rows / K tail are zero-filled by TMA.
+//   warpgroups 1..TEAMS: consumers.  Tile i of the CTA belongs to consumer i % TEAMS, which runs
+//                        the wgmma main loop (m64 x n16 x k16, fp32 accumulators in registers) and
+//                        then its own epilogue: +bias -> activation -> (+residual) -> fp16 ->
+//                        128B-swizzled staging slab -> TMA store (clips the ragged M / N edges).
+//                        While one consumer is in its MUFU-bound epilogue the other one's MMAs run.
 //
 // Replaces Conv2D 1x1 (+BN, +swish, +skip) at the reference call sites listed in
 // include/automl_b200.h (edet_pointwise_conv).  Algorithmic HBM bytes per launch:
@@ -26,36 +26,29 @@
 namespace edet {
 namespace pwtc {
 
-// warp 0 TMA, warp 1 MMA, then TEAMS x 4 epilogue warps (one per TMEM lane quarter and team):
-//   TEAMS == 2: 320 threads, <= 96 registers; every 64-column store chunk is split between the
-//               two teams' staging slabs (4 KiB each)
-//   TEAMS == 3: 448 threads, <= 72 registers; the unit of epilogue work is 32 columns (one
-//               2 KiB [32 rows x 32 cols] TMA store), handed to the teams round robin -- 50 % more
-//               warps to hide the MUFU / dependent-issue latency of the swish epilogue, balanced
-//               for the expand widths (N = 96, 144, 240 and tiles of 96)
+constexpr int BLOCK_M = 64;         // rows per tile = the M of one wgmma
+constexpr int kMaxBlockN = 128;     // accumulator columns per consumer thread: kMaxBlockN / 2
+constexpr int kNT = kMaxBlockN / 16;
 template <int TEAMS>
 struct Epi {
-  static constexpr int kWarps = 4 * TEAMS;
-  static constexpr int kThreads = 64 + 32 * kWarps;
-  static constexpr int kSlabBytes = TEAMS == 2 ? 4096 : 2048;
+  static constexpr int kThreads = 128 * (1 + TEAMS);
 };
 constexpr int kStoreCols = 64;
-constexpr int kMaxStages = 8;
+constexpr int kSlabBytes = BLOCK_M * kStoreCols * 2;   // [64 rows][64 cols] fp16, 128B swizzle
+constexpr int kSlabsPerTeam = kMaxBlockN / kStoreCols;
+constexpr int kMaxStages = 9;   // 4 + 4 (two consumers) or 3 + 3 + 3
 constexpr int kRing = 4;          // tile-index ring entries (power of two)
-constexpr int kMaxAccum = 4;      // TMEM accumulator stages (thin N tiles)
-constexpr int kSmemLimit = 113 * 1024;                    // two CTAs per SM share the 227 KiB
-constexpr int kSmemCoResident = 99 * 1024;               // one CTA next to an nms_v5_fast CTA
+constexpr int kSmemLimit = 227 * 1024;                   // one CTA per SM
 
 struct Params {
   int batch, rows, k, nout, nout_pad8;
   int block_n, num_m_blocks, num_n_blocks, num_k_blocks, num_stages;
+  int team_stages;    // stages of each consumer's own ring: num_stages / TEAMS
   int block_k;        // 64 / 32 / 16 halves per k-block == 128B / 64B / 32B swizzled smem rows
   int a_stage_bytes, b_stage_bytes;
   int desc_sbo;       // byte distance between 8-row groups in smem (8 * row pitch)
-  int desc_layout;    // UMMA layout type: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
-  int slabs_per_warp; // private TMA-store staging slabs per epilogue warp (1 or 2)
-  int accum_stages;   // TMEM accumulator stages: 1..kMaxAccum, accum_stages * block_n <= 256 columns
-  int wbatch, ldr, tmem_cols;
+  int desc_layout;    // wgmma layout type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
+  int wbatch, ldr;
   int total_tiles;
   int bias_floats;    // floats of the zero-padded bias staged in shared memory: whole N tiles
   const float* bias;
@@ -72,27 +65,7 @@ constexpr int kArgmaxCols = 96;   // columns per anchor in the padded class-head
 struct TileCoord {
   int b, m_blk, n_blk;
 };
-// (accumulator stage, mbarrier phase) of consecutive tiles without a division per tile
-struct StageCounter {
-  int as = -1;
-  uint32_t phase = 1u;
-  __device__ __forceinline__ void next(int stages) {
-    if (++as == stages) as = 0;
-    if (as == 0) phase ^= 1u;
-  }
-};
-// Biases of 8 consecutive output columns from the copy of the (zero-padded) bias vector that the
-// prologue stages in shared memory: two ld.shared.v4 instead of two global loads plus the
-// ragged-edge branches in the middle of the MUFU / issue-bound epilogue.
 constexpr int kMaxBiasSmem = 8192;
-__device__ __forceinline__ void load_bias8(uint32_t smem_bias_u32, int col, float4& b0, float4& b1) {
-  const uint32_t a = smem_bias_u32 + static_cast<uint32_t>(col) * 4u;
-  // not volatile: the staged bias is constant for the kernel, so the loads may move freely
-  asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-      : "=f"(b0.x), "=f"(b0.y), "=f"(b0.z), "=f"(b0.w) : "r"(a));
-  asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-      : "=f"(b1.x), "=f"(b1.y), "=f"(b1.z), "=f"(b1.w) : "r"(a + 16u));
-}
 
 __device__ __forceinline__ TileCoord decode_tile(int t, const Params& p) {
   TileCoord c;
@@ -110,8 +83,26 @@ __device__ __forceinline__ TileCoord decode_tile(int t, const Params& p) {
   return c;
 }
 
+// Running arg-max key of a pair of adjacent logits (columns col, col + 1): each logit is rounded
+// to fp16 exactly as the storing epilogue would store it and mapped to an order-preserving uint16,
+// << 16 | (0xFFFF - column), so that one unsigned max gives the maximum AND its first column
+// (equal logits: the lower column has the larger key).  -0 is canonicalised to +0 first (the
+// float compare of the stored-logits path treats them as equal).
+__device__ __forceinline__ uint32_t argmax_pair_key(float2 s, uint32_t col) {
+  const __half2 h = __hadd2(__floats2half2_rn(s.x, s.y), __float2half2_rn(0.f));
+  const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h);
+  uint32_t sgn;      // 0xFFFF in the halves that are negative
+  asm("prmt.b32 %0, %1, %2, 0xBB99;" : "=r"(sgn) : "r"(hb), "r"(0u));
+  const uint32_t ord = hb ^ (sgn | 0x80008000u);       // order-preserving uint16 x 2
+  const uint32_t codes = ((0xFFFFu - (col + 1u)) << 16) | (0xFFFFu - col);
+  uint32_t k0, k1;
+  asm("prmt.b32 %0, %1, %2, 0x1054;" : "=r"(k0) : "r"(ord), "r"(codes));
+  asm("prmt.b32 %0, %1, %2, 0x3276;" : "=r"(k1) : "r"(ord), "r"(codes));
+  return max(k0, k1);
+}
+
 template <int ACT, bool HAS_RES, int TEAMS, int EPI>
-__global__ void __launch_bounds__(Epi<TEAMS>::kThreads, 2)
+__global__ void __launch_bounds__(Epi<TEAMS>::kThreads, 1)
 pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
                     const __grid_constant__ CUtensorMap map_w,
                     const __grid_constant__ CUtensorMap map_o, const Params p) {
@@ -121,26 +112,20 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
-  uint8_t* smem_store = smem + p.num_stages * stage_bytes;
-  constexpr int kEpiWarps = Epi<TEAMS>::kWarps;
-  constexpr int kSlabBytes = Epi<TEAMS>::kSlabBytes;
-  float* smem_bias = reinterpret_cast<float*>(smem_store + p.slabs_per_warp * kEpiWarps * kSlabBytes);
+  uint8_t* smem_store = smem + p.num_stages * stage_bytes;   // [TEAMS][kSlabsPerTeam] slabs
+  float* smem_bias = reinterpret_cast<float*>(smem_store + TEAMS * kSlabsPerTeam * kSlabBytes);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_bias + p.bias_floats);
-  const uint32_t smem_bias_u32 = smem_u32(smem_bias);
   uint64_t* full_bar = bars;                       // [kMaxStages]
   uint64_t* empty_bar = bars + kMaxStages;         // [kMaxStages]
-  uint64_t* tmem_full_bar = bars + 2 * kMaxStages;                 // [kMaxAccum]
-  uint64_t* tmem_empty_bar = bars + 2 * kMaxStages + kMaxAccum;    // [kMaxAccum]
-  // Tile indices travel from the producer to the MMA warp and the epilogue warps through a small
-  // ring: CTA i owns tile i, every further tile comes from a global counter (sched_next_tile), so
-  // a CTA that gets its SM late -- another stream's kernel, e.g. the NMS of the previous batch,
-  // was holding it -- simply finds less work instead of owning a full static share.
-  uint64_t* ring_full = bars + 2 * kMaxStages + 2 * kMaxAccum;   // [kRing] producer -> consumers
-  uint64_t* ring_empty = ring_full + kRing;              // [kRing] consumers -> producer
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ring_empty + kRing);
+  // Tile indices travel from the producer to the consumers through a small ring: CTA i owns tile
+  // i, every further tile comes from a global counter (sched_next_tile), so a CTA that gets its
+  // SM late -- another stream's kernel, e.g. the NMS of the previous batch, was holding it --
+  // simply finds less work instead of owning a full static share.
+  uint64_t* ring_full = bars + 2 * kMaxStages;     // [kRing] producer -> consumers
+  uint64_t* ring_empty = ring_full + kRing;        // [kRing] consumers -> producer
   // [kRing] x {tile, batch entry, M block, N block}: the producer decodes each tile once (its two
-  // integer divisions) and the 13 consumer warps read the coordinates with one 16-byte load
-  volatile int4* tile_ring = reinterpret_cast<volatile int4*>(tmem_slot + 4);
+  // integer divisions) and the consumers read the coordinates with one 16-byte load
+  volatile int4* tile_ring = reinterpret_cast<volatile int4*>(ring_empty + kRing);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -148,15 +133,11 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.num_stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
-    }
-    for (int s = 0; s < kMaxAccum; ++s) {
-      mbar_init(smem_u32(&tmem_full_bar[s]), 1);
-      mbar_init(smem_u32(&tmem_empty_bar[s]), kEpiWarps);  // one arrive per epilogue warp
+      mbar_init(smem_u32(&empty_bar[s]), 4);       // one arrive per warp of the consumer
     }
     for (int s = 0; s < kRing; ++s) {
       mbar_init(smem_u32(&ring_full[s]), 1);
-      mbar_init(smem_u32(&ring_empty[s]), 1 + kEpiWarps);  // the MMA warp + every epilogue warp
+      mbar_init(smem_u32(&ring_empty[s]), TEAMS);  // one arrive per consumer warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
@@ -166,40 +147,13 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
   // bias (a constant, like the weights: read before the PDL wait) -> shared memory, zero padded
   for (int i = threadIdx.x; i < p.bias_floats; i += blockDim.x)
     smem_bias[i] = i < p.nout ? __ldg(p.bias + i) : 0.f;
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait_prior();          // everything above overlapped the previous kernel's tail
-
-  // consumer side of the tile ring: whole warp (or the single MMA lane) waits, reads, releases
-  auto ring_get = [&](int i, bool whole_warp, TileCoord* tc) -> int {
-    const int slot = i & (kRing - 1);
-    mbar_wait(smem_u32(&ring_full[slot]), static_cast<uint32_t>(i / kRing) & 1u);
-    const int4 e = const_cast<const int4*>(tile_ring)[slot];
-    if (whole_warp) __syncwarp();
-    if (!whole_warp || lane == 0) mbar_arrive(smem_u32(&ring_empty[slot]));
-    if (tc) {
-      tc->b = e.y;
-      tc->m_blk = e.z;
-      tc->n_blk = e.w;
-    }
-    return e.x;
-  };
 
   if (warp == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+      int stage_of[TEAMS] = {}, phase_of[TEAMS] = {};   // per consumer ring
       // bytes the two TMA boxes deliver (the B slot may be padded to 1 KiB)
       const uint32_t tx_bytes = static_cast<uint32_t>(p.a_stage_bytes + p.block_n * p.block_k * 2);
       bool exhausted = false;
@@ -220,388 +174,182 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
         mbar_arrive(smem_u32(&ring_full[slot]));     // release: the entry is visible to waiters
         if (t >= p.total_tiles) break;
         const int wb = (p.wbatch > 1) ? tc.b : 0;
+        const int team = i % TEAMS;
+        int stage = stage_of[team];
+        uint32_t phase = static_cast<uint32_t>(phase_of[team]);
         for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          mbar_wait(smem_u32(&empty_bar[stage]), phase ^ 1);
-          const uint32_t fb = smem_u32(&full_bar[stage]);
+          const int s = team * p.team_stages + stage;
+          mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
+          const uint32_t fb = smem_u32(&full_bar[s]);
           mbar_expect_tx(fb, tx_bytes);
-          uint8_t* sa = smem + stage * stage_bytes;
+          uint8_t* sa = smem + s * stage_bytes;
           tma_load_3d(smem_u32(sa), &map_a, fb, kb * p.block_k, tc.m_blk * BLOCK_M, tc.b);
           tma_load_3d(smem_u32(sa + p.a_stage_bytes), &map_w, fb, kb * p.block_k,
                       tc.n_blk * p.block_n, wb);
-          if (++stage == p.num_stages) {
+          if (++stage == p.team_stages) {
             stage = 0;
             phase ^= 1;
           }
         }
+        stage_of[team] = stage;
+        phase_of[team] = static_cast<int>(phase);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      // cute::UMMA::InstrDescriptor: c_format F32 (1<<4), a/b F16 (0), K-major both,
-      // n_dim = N>>3 at bit 17, m_dim = M>>4 at bit 24.
-      const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(p.block_n >> 3) << 17) |
-                             (static_cast<uint32_t>(BLOCK_M >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      StageCounter sc;
-      for (int iter = 0;; ++iter) {
-        if (ring_get(iter, false, nullptr) >= p.total_tiles) break;
-        sc.next(p.accum_stages);
-        const int as = sc.as;
-        const uint32_t aphase = sc.phase;
-        mbar_wait(smem_u32(&tmem_empty_bar[as]), aphase ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(as * p.block_n);
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          mbar_wait(smem_u32(&full_bar[stage]), phase);
-          tc_fence_after();
-          uint8_t* sa = smem + stage * stage_bytes;
-          const uint64_t da = make_smem_desc(smem_u32(sa), p.desc_sbo, p.desc_layout);
-          const uint64_t db = make_smem_desc(smem_u32(sa + p.a_stage_bytes), p.desc_sbo, p.desc_layout);
-          const int k_rem = p.k - kb * p.block_k;
-          const int ksteps = k_rem >= p.block_k ? p.block_k / UMMA_K : (k_rem + UMMA_K - 1) / UMMA_K;
-          for (int ks = 0; ks < ksteps; ++ks) {
-            // advance 16 halves = 32 bytes inside the swizzle atom: +2 in the >>4 address field
-            tc_mma_f16(tmem_d, da + static_cast<uint64_t>(ks * 2), db + static_cast<uint64_t>(ks * 2),
-                       idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-          }
-          tc_commit(smem_u32(&empty_bar[stage]));  // frees the smem stage when the MMAs retire
-          if (++stage == p.num_stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        tc_commit(smem_u32(&tmem_full_bar[as]));  // accumulator ready for the epilogue
+  } else if (warp >= 4) {
+    // ===================== consumers: MMA + epilogue =====================
+    const int team = (warp >> 2) - 1;
+    const int wtid = threadIdx.x & 127;
+    const int r0 = 16 * (warp & 3) + (lane >> 2);   // rows r0 and r0 + 8 of the tile
+    const int cq = 2 * (lane & 3);                  // column pair inside each 8-column group
+    uint8_t* my_slabs = smem_store + team * kSlabsPerTeam * kSlabBytes;
+    const int b_chunk = p.block_k * 2;              // descriptor units between 16-row B chunks
+    int stage = 0;            // in this consumer's ring: stages team * team_stages ..
+    uint32_t phase = 0;
+    auto advance = [&]() {
+      if (++stage == p.team_stages) {
+        stage = 0;
+        phase ^= 1;
       }
-    }
-  } else {
-    // ===================== Epilogue =====================
-    if constexpr (TEAMS == 2) {
-    // Fully decoupled warps: warp (quarter, team) owns rows quarter*32..+31 of the tile and the
-    // 64-column store chunks c == team (mod 2).  Each warp has a private 4 KiB staging slab and
-    // issues its own TMA stores ([32 rows x 64 cols] boxes), so the only synchronisation in the
-    // epilogue is the TMEM full/empty handshake with the MMA warp.
-    const int e_warp = warp - 2;              // 0..7
-    const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-    const int team = e_warp >> 2;             // even / odd store chunks
-    const int row_in_tile = quarter * 32 + lane;
-    uint8_t* my_slabs = smem_store + e_warp * p.slabs_per_warp * (32 * 128);
-    int store_cnt = 0;
-    StageCounter sc;
+    };
     for (int iter = 0;; ++iter) {
-      TileCoord tc;
-      const int t = ring_get(iter, true, &tc);
+      const int slot = iter & (kRing - 1);
+      mbar_wait(smem_u32(&ring_full[slot]), static_cast<uint32_t>(iter / kRing) & 1u);
+      const int4 e = const_cast<const int4*>(tile_ring)[slot];
+      named_sync(1 + team, 128);
+      if (wtid == 0) mbar_arrive(smem_u32(&ring_empty[slot]));
+      const int t = e.x;
       if (t >= p.total_tiles) break;
-      sc.next(p.accum_stages);
-      const int as = sc.as;
-      const uint32_t aphase = sc.phase;
+      if (iter % TEAMS != team) continue;   // another consumer's tile (and ring)
+      TileCoord tc;
+      tc.b = e.y;
+      tc.m_blk = e.z;
+      tc.n_blk = e.w;
       const int n0 = tc.n_blk * p.block_n;
-      const int row = tc.m_blk * BLOCK_M + row_in_tile;
-      const bool row_ok = row < p.rows;
-      const __half* res_row = nullptr;
-      if (HAS_RES) {
-        res_row = p.residual + (static_cast<size_t>(tc.b) * p.rows + (row_ok ? row : 0)) * p.ldr;
-      }
-      mbar_wait(smem_u32(&tmem_full_bar[as]), aphase);
-      tc_fence_after();
-      // only the columns that exist in the output are worth an epilogue (rounded up to the
-      // 16-column TMEM load granule); the rest of a ragged last N tile is skipped
+      // only the columns that exist in the output are worth MMAs and an epilogue (rounded up to
+      // the 16-column MMA granule); the rest of a ragged last N tile is skipped
       const int n_valid = min(p.block_n, ((p.nout - n0 + 15) >> 4) << 4);
-      const int num_chunks = (n_valid + kStoreCols - 1) / kStoreCols;
-      // last chunk this warp reads from TMEM (then the accumulator can be handed back)
-      int my_last = -1;
-      for (int c = team; c < num_chunks; c += 2) my_last = c;
-      if (my_last < 0) {
-        tc_fence_before();
+      const int nt = n_valid >> 4;
+      float acc[kNT][8];
+#pragma unroll
+      for (int j = 0; j < kNT; ++j)
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[j][q] = 0.f;
+      for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+        const int s = team * p.team_stages + stage;
+        mbar_wait(smem_u32(&full_bar[s]), phase);
+        uint8_t* sa = smem + s * stage_bytes;
+        const uint64_t da = make_smem_desc(smem_u32(sa), p.desc_sbo, p.desc_layout);
+        const uint64_t db = make_smem_desc(smem_u32(sa + p.a_stage_bytes), p.desc_sbo, p.desc_layout);
+        const int k_rem = p.k - kb * p.block_k;
+        const int ksteps = k_rem >= p.block_k ? p.block_k / MMA_K : (k_rem + MMA_K - 1) / MMA_K;
+        wg_fence();
+        wg_mma_kblock<kNT>(acc, da, db, b_chunk, nt, ksteps, kb == 0);
+        wg_commit();
+        wg_wait<0>();
         __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
+        if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));   // this warp is done with it
+        advance();
       }
-      for (int c = team; c < num_chunks; c += 2) {
-        const int cols = min(kStoreCols, n_valid - c * kStoreCols);  // multiple of 16
-        uint8_t* my_stage = my_slabs + (p.slabs_per_warp == 2 ? (store_cnt & 1) * 4096 : 0);
-        ++store_cnt;
-        if (lane == 0) {                           // the store that last used this slab has left it
-          if (p.slabs_per_warp == 2) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
+      wg_fence_acc<kNT>(acc);
+      const int row0 = tc.m_blk * BLOCK_M + r0;
+      if constexpr (EPI == EPI_ARGMAX) {
+        // Class head fused with the class half of pre-NMS (tf2/postprocess.py:88-156 with
+        // max_nms_inputs == 0): an N tile is ONE anchor (90 class columns + 6 pad columns whose
+        // bias is -inf).  Each logit is rounded to fp16 exactly as the storing epilogue would
+        // store it, then max / first arg-max / sigmoid as pre_nms_kernel does -> bit-identical
+        // scores and classes, without the [N, H, W, 810] logits ever reaching HBM.
+        const float* bias = smem_bias + tc.n_blk * kArgmaxCols;
+        uint32_t best[2] = {0u, 0u};                  // rows r0, r0 + 8
+#pragma unroll
+        for (int j = 0; j < kArgmaxCols / 16; ++j) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int col = 16 * j + 8 * h + cq;
+            const float2 b = *reinterpret_cast<const float2*>(bias + col);
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              const float2 s = fadd2_rn(make_float2(acc[j][4 * h + 2 * r], acc[j][4 * h + 2 * r + 1]), b);
+              best[r] = max(best[r], argmax_pair_key(s, static_cast<uint32_t>(col)));
+            }
+          }
         }
-        __syncwarp();
-        uint8_t* row_base = my_stage + lane * 128;
 #pragma unroll
-        for (int hf = 0; hf < 2; ++hf) {
-          const int c_lo = hf * 32;
-          if (c_lo >= cols) break;
-          float v[32];
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) +
-                                 static_cast<uint32_t>(as * p.block_n + c * kStoreCols + c_lo);
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            if (c_lo + g * 16 < cols) tc_ld16(taddr + g * 16, v + g * 16);
+        for (int r = 0; r < 2; ++r) {      // the four lanes of a quad hold the same row
+          best[r] = max(best[r], __shfl_xor_sync(0xffffffffu, best[r], 1));
+          best[r] = max(best[r], __shfl_xor_sync(0xffffffffu, best[r], 2));
+          const uint32_t ord_best = best[r] >> 16;
+          const unsigned short hbits = static_cast<unsigned short>(
+              (ord_best & 0x8000u) ? (ord_best ^ 0x8000u) : (~ord_best & 0xFFFFu));
+          const float bv = __half2float(__ushort_as_half(hbits));
+          const int best_c = static_cast<int>(0xFFFFu - (best[r] & 0xFFFFu));
+          const int row = row0 + 8 * r;
+          if ((lane & 3) == 0 && row < p.rows) {
+            const size_t o = static_cast<size_t>(tc.b) * p.am_total + p.am_anchor_begin +
+                             static_cast<size_t>(row) * p.am_num_anchors + tc.n_blk;
+            p.am_scores[o] = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-bv)));
+            p.am_classes[o] = best_c;
           }
-          tc_wait_ld();
-          if (c == my_last && (hf == 1 || c_lo + 32 >= cols)) {
-            // all TMEM reads of this warp for this accumulator are done
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
-          }
+        }
+      } else {
+        const bool ok[2] = {row0 < p.rows, row0 + 8 < p.rows};
+        const __half* res_row[2] = {nullptr, nullptr};
+        if (HAS_RES) {
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            if (c_lo + jj * 8 < cols) {
-              const int col = n0 + c * kStoreCols + c_lo + jj * 8;
-              float4 b0, b1;
-              load_bias8(smem_bias_u32, col, b0, b1);
-              float2 o2[4];
-              o2[0] = __fadd2_rn(make_float2(v[jj * 8 + 0], v[jj * 8 + 1]), make_float2(b0.x, b0.y));
-              o2[1] = __fadd2_rn(make_float2(v[jj * 8 + 2], v[jj * 8 + 3]), make_float2(b0.z, b0.w));
-              o2[2] = __fadd2_rn(make_float2(v[jj * 8 + 4], v[jj * 8 + 5]), make_float2(b1.x, b1.y));
-              o2[3] = __fadd2_rn(make_float2(v[jj * 8 + 6], v[jj * 8 + 7]), make_float2(b1.z, b1.w));
-              apply_act4<ACT>(o2[0], o2[1]);
-              apply_act4<ACT>(o2[2], o2[3]);
-              float o[8] = {o2[0].x, o2[0].y, o2[1].x, o2[1].y, o2[2].x, o2[2].y, o2[3].x, o2[3].y};
-              if (HAS_RES) {
-                if (row_ok && col < p.nout) {
-                  float r[8];
-                  half8_to_float(ldg_nc_v4(res_row + col), r);
+          for (int r = 0; r < 2; ++r)
+            res_row[r] = p.residual +
+                         (static_cast<size_t>(tc.b) * p.rows + (ok[r] ? row0 + 8 * r : 0)) * p.ldr;
+        }
+        // the slabs are free once this consumer's previous stores have read them
+        if (wtid == 0) tma_store_wait_read<0>();
+        named_sync(1 + team, 128);
 #pragma unroll
-                  for (int e = 0; e < 8; ++e) o[e] += r[e];
-                }
+        for (int j = 0; j < kNT; ++j) {
+          if (j < nt) {
+            const int colt = 16 * j + cq;            // tile column of acc[j][0]
+            const float2 b_lo = *reinterpret_cast<const float2*>(smem_bias + n0 + colt);
+            const float2 b_hi = *reinterpret_cast<const float2*>(smem_bias + n0 + colt + 8);
+            uint8_t* slab = my_slabs + (colt >> 6) * kSlabBytes;
+            const int piece = (colt & 63) >> 3;      // 16-byte piece of the 128-byte slab row
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              float2 lo = fadd2_rn(make_float2(acc[j][2 * r], acc[j][2 * r + 1]), b_lo);
+              float2 hi = fadd2_rn(make_float2(acc[j][4 + 2 * r], acc[j][4 + 2 * r + 1]), b_hi);
+              apply_act4<ACT>(lo, hi);
+              if (HAS_RES && ok[r]) {
+                const int col = n0 + colt;
+                if (col < p.nout)
+                  lo = fadd2_rn(lo, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col)));
+                if (col + 8 < p.nout)
+                  hi = fadd2_rn(hi, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col + 8)));
               }
-              const uint4 packed = float_to_half8(o);
-              const int chunk16 = hf * 4 + jj;   // 16-byte piece inside the 128-byte row
-              *reinterpret_cast<uint4*>(row_base + ((chunk16 ^ (lane & 7)) << 4)) = packed;
+              const int row = r0 + 8 * r;
+              uint8_t* rb = slab + row * 128 + cq * 2;
+              *reinterpret_cast<__half2*>(rb + ((piece ^ (row & 7)) << 4)) = __floats2half2_rn(lo.x, lo.y);
+              *reinterpret_cast<__half2*>(rb + (((piece + 1) ^ (row & 7)) << 4)) = __floats2half2_rn(hi.x, hi.y);
             }
           }
         }
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_3d(&map_o, smem_u32(my_stage), n0 + c * kStoreCols,
-                       tc.m_blk * BLOCK_M + quarter * 32, tc.b);
+        named_sync(1 + team, 128);
+        if (wtid == 0) {
+          for (int c = 0; c * kStoreCols < n_valid; ++c)
+            tma_store_3d(&map_o, smem_u32(my_slabs + c * kSlabBytes), n0 + c * kStoreCols,
+                         tc.m_blk * BLOCK_M, tc.b);
           tma_store_commit();
         }
       }
     }
-    } else if constexpr (EPI == EPI_ARGMAX) {
-      // Class head fused with the class half of pre-NMS (tf2/postprocess.py:88-156 with
-      // max_nms_inputs == 0): an N tile is ONE anchor (90 class columns + 6 pad columns whose
-      // staged bias is -inf); the team (iter % TEAMS) owns the whole tile, lane = pixel.  Each
-      // logit is rounded to fp16 exactly as the storing epilogue would store it, then max / first
-      // arg-max / sigmoid as pre_nms_kernel does -> bit-identical scores and classes, without the
-      // [N, H, W, 810] logits ever reaching HBM.
-      const int e_warp = warp - 2;
-      const int quarter = warp & 3;
-      const int team = e_warp >> 2;
-      const int row_in_tile = quarter * 32 + lane;
-      StageCounter sc;
-      int rot = TEAMS - 1;                      // iter % TEAMS, kept incrementally
-      for (int iter = 0;; ++iter) {
-        TileCoord tc;
-        const int t = ring_get(iter, true, &tc);
-        if (t >= p.total_tiles) break;
-        sc.next(p.accum_stages);
-        if (++rot == TEAMS) rot = 0;
-        const int as = sc.as;
-        const uint32_t aphase = sc.phase;
-        mbar_wait(smem_u32(&tmem_full_bar[as]), aphase);
-        tc_fence_after();
-        if (rot != team) {                       // not this team's tile: hand the accumulator back
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
-          continue;
-        }
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) +
-                               static_cast<uint32_t>(as * p.block_n);
-        const uint32_t bias_u32 = smem_bias_u32 + static_cast<uint32_t>(tc.n_blk * kArgmaxCols) * 4u;
-        // Running maximum over 32-bit keys (fp16 logit mapped to an order-preserving uint16) << 16 |
-        // (0xFFFF - column): one unsigned max per column pair gives the maximum AND its first
-        // column (equal logits: the lower column has the larger key), with no serial
-        // compare / select chain.  -0 is canonicalised to +0 first (the float compare of the
-        // stored-logits path treats them as equal).
-        uint32_t best_key = 0u;
-#pragma unroll
-        for (int g = 0; g < kArgmaxCols / 16; ++g) {
-          float v[16];
-          tc_ld16(taddr + g * 16, v);
-          tc_wait_ld();
-          if (g == kArgmaxCols / 16 - 1) {       // all TMEM reads of this warp are done
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float4 b;
-            asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                : "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w)
-                : "r"(bias_u32 + static_cast<uint32_t>(g * 16 + q * 4) * 4u));
-            const float2 s01 = __fadd2_rn(make_float2(v[q * 4 + 0], v[q * 4 + 1]), make_float2(b.x, b.y));
-            const float2 s23 = __fadd2_rn(make_float2(v[q * 4 + 2], v[q * 4 + 3]), make_float2(b.z, b.w));
-            const float2 pairs[2] = {s01, s23};
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              // the two logits exactly as the storing epilogue rounds them; -0 -> +0
-              const __half2 h = __hadd2(__floats2half2_rn(pairs[e].x, pairs[e].y), __float2half2_rn(0.f));
-              const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h);
-              uint32_t sgn;      // 0xFFFF in the halves that are negative
-              asm("prmt.b32 %0, %1, %2, 0xBB99;" : "=r"(sgn) : "r"(hb), "r"(0u));
-              const uint32_t ord = hb ^ (sgn | 0x80008000u);       // order-preserving uint16 x 2
-              // (0xFFFF - col) of the pair's two columns in one register; selectors as immediates
-              const uint32_t col = static_cast<uint32_t>(g * 16 + q * 4 + e * 2);
-              const uint32_t codes = ((0xFFFFu - (col + 1u)) << 16) | (0xFFFFu - col);
-              uint32_t k0, k1;
-              asm("prmt.b32 %0, %1, %2, 0x1054;" : "=r"(k0) : "r"(ord), "r"(codes));
-              asm("prmt.b32 %0, %1, %2, 0x3276;" : "=r"(k1) : "r"(ord), "r"(codes));
-              best_key = max(best_key, max(k0, k1));
-            }
-          }
-        }
-        const uint32_t ord_best = best_key >> 16;
-        const unsigned short hbits = static_cast<unsigned short>(
-            (ord_best & 0x8000u) ? (ord_best ^ 0x8000u) : (~ord_best & 0xFFFFu));
-        const float best = __half2float(__ushort_as_half(hbits));
-        const int best_c = static_cast<int>(0xFFFFu - (best_key & 0xFFFFu));
-        const int row = tc.m_blk * BLOCK_M + row_in_tile;
-        if (row < p.rows) {
-          const size_t o = static_cast<size_t>(tc.b) * p.am_total + p.am_anchor_begin +
-                           static_cast<size_t>(row) * p.am_num_anchors + tc.n_blk;
-          p.am_scores[o] = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-best)));
-          p.am_classes[o] = best_c;
-        }
-      }
-    } else {
-      // Units of 32 columns: warp (quarter, team) owns rows quarter*32..+31 of the tile and the
-      // units u == team (mod TEAMS).  Each warp has private 2 KiB staging slabs ([32 rows] x 64
-      // bytes, 64B-swizzled) and issues its own [32 x 32] TMA stores; the only synchronisation is
-      // the TMEM full / empty handshake with the MMA warp.
-      const int e_warp = warp - 2;
-      const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-      const int team = e_warp >> 2;
-      const int row_in_tile = quarter * 32 + lane;
-      uint8_t* my_slabs = smem_store + e_warp * p.slabs_per_warp * kSlabBytes;
-      int store_cnt = 0;
-      StageCounter sc;
-      int rot = TEAMS - 1;                      // iter % TEAMS, kept incrementally
-      for (int iter = 0;; ++iter) {
-        TileCoord tc;
-        const int t = ring_get(iter, true, &tc);
-        if (t >= p.total_tiles) break;
-        sc.next(p.accum_stages);
-        if (++rot == TEAMS) rot = 0;
-        const int as = sc.as;
-        const uint32_t aphase = sc.phase;
-        const int n0 = tc.n_blk * p.block_n;
-        const int row = tc.m_blk * BLOCK_M + row_in_tile;
-        const bool row_ok = row < p.rows;
-        const __half* res_row = nullptr;
-        if (HAS_RES) {
-          res_row = p.residual + (static_cast<size_t>(tc.b) * p.rows + (row_ok ? row : 0)) * p.ldr;
-        }
-        mbar_wait(smem_u32(&tmem_full_bar[as]), aphase);
-        tc_fence_after();
-        const int n_valid = min(p.block_n, ((p.nout - n0 + 15) >> 4) << 4);
-        const int num_units = (n_valid + 31) >> 5;
-        // unit u of tile `iter` belongs to team (u + iter) % TEAMS: thin layers (one or two units
-        // per tile) keep all three teams busy on consecutive tiles (up to kMaxAccum accumulators
-        // in flight) instead of leaving two of them idle
-        const int u_first = team >= rot ? team - rot : team + TEAMS - rot;
-        int my_last = -1;
-        for (int u = u_first; u < num_units; u += TEAMS) my_last = u;
-        if (my_last < 0) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
-        }
-        for (int u = u_first; u < num_units; u += TEAMS) {
-          const int cols = min(32, n_valid - u * 32);      // 16 or 32
-          uint8_t* my_stage = my_slabs + (p.slabs_per_warp == 2 ? (store_cnt & 1) * kSlabBytes : 0);
-          ++store_cnt;
-          if (lane == 0) {                        // the store that last used this slab has left it
-            if (p.slabs_per_warp == 2) tma_store_wait_read<1>(); else tma_store_wait_read<0>();
-          }
-          __syncwarp();
-          const uint32_t row_base = smem_u32(my_stage) + lane * 64;
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) +
-                                 static_cast<uint32_t>(as * p.block_n + u * 32);
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            if (g * 16 < cols) {
-              float v[16];
-              tc_ld16(taddr + g * 16, v);
-              tc_wait_ld();
-              if (u == my_last && (g == 1 || cols == 16)) {
-                // all TMEM reads of this warp for this accumulator are done
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(smem_u32(&tmem_empty_bar[as]));
-              }
-#pragma unroll
-              for (int jj = 0; jj < 2; ++jj) {
-                const int col = n0 + u * 32 + g * 16 + jj * 8;
-                float4 b0, b1;
-                load_bias8(smem_bias_u32, col, b0, b1);
-                float2 o2[4];
-                o2[0] = __fadd2_rn(make_float2(v[jj * 8 + 0], v[jj * 8 + 1]), make_float2(b0.x, b0.y));
-                o2[1] = __fadd2_rn(make_float2(v[jj * 8 + 2], v[jj * 8 + 3]), make_float2(b0.z, b0.w));
-                o2[2] = __fadd2_rn(make_float2(v[jj * 8 + 4], v[jj * 8 + 5]), make_float2(b1.x, b1.y));
-                o2[3] = __fadd2_rn(make_float2(v[jj * 8 + 6], v[jj * 8 + 7]), make_float2(b1.z, b1.w));
-                apply_act4<ACT>(o2[0], o2[1]);
-                apply_act4<ACT>(o2[2], o2[3]);
-                float o[8] = {o2[0].x, o2[0].y, o2[1].x, o2[1].y, o2[2].x, o2[2].y, o2[3].x, o2[3].y};
-                if (HAS_RES) {
-                  if (row_ok && col < p.nout) {
-                    float r[8];
-                    half8_to_float(ldg_nc_v4(res_row + col), r);
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) o[e] += r[e];
-                  }
-                }
-                const uint4 packed = float_to_half8(o);
-                const int chunk16 = g * 2 + jj;    // 16-byte piece inside the 64-byte row
-                // 64B swizzle: the 16-byte piece index is XORed with bits [7:8] of the address
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(
-                                 row_base + (((chunk16 ^ ((lane >> 1) & 3))) << 4)),
-                             "r"(packed.x), "r"(packed.y), "r"(packed.z), "r"(packed.w)
-                             : "memory");
-              }
-            }
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_3d(&map_o, smem_u32(my_stage), n0 + u * 32, tc.m_blk * BLOCK_M + quarter * 32,
-                         tc.b);
-            tma_store_commit();
-          }
-        }
-      }
-    }
-    if (lane == 0) tma_store_wait_all();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
+    if (wtid == 0) tma_store_wait_all();
   }
 }
 
-// N tile.  Two CTAs are resident per SM (<=113 KiB smem, <=256 TMEM columns each):
-//   nout <= 128 : one tile, two accumulator stages;
-//   nout <= 256 : one tile, ONE accumulator stage (the other CTA of the SM hides the gap) --
-//                 avoids re-reading A and a ragged second tile for N = 144 / 240 (splitting these
-//                 into two double-buffered tiles measured 1.5 % slower on the D0 step);
-//   wider       : tiles of 128 columns; the A tile of the extra tiles comes from L2 and the
-//                 epilogue skips the columns past nout.
-// With three epilogue teams (32-column units) wide layers use tiles of 96 columns (3 units).
-static int pick_block_n(int nout, int teams) {
-  if (nout <= 128) return ((nout + 15) / 16) * 16;
-  if (nout <= 256) return ((nout + 15) / 16) * 16;
-  return teams == 3 ? 96 : 128;
+// N tile: the whole width up to kMaxBlockN (one tile, A read once); wider layers use tiles of
+// 128 columns (a multiple of the 64-column store box, so that a tile's stores never reach into
+// the next tile), the A tile of the extra tiles comes from L2.  The class-head arg-max epilogue
+// needs one anchor (kArgmaxCols columns) per tile.
+static int pick_block_n(int nout) {
+  if (nout <= kMaxBlockN) return ((nout + 15) / 16) * 16;
+  return kMaxBlockN;
 }
 
 template <int ACT, bool HAS_RES, int TEAMS, int EPI = EPI_STORE>
@@ -633,82 +381,46 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   p.k = k;
   p.nout = nout;
   p.nout_pad8 = nout & ~7;   // whole float4 pairs of bias that are in bounds
-  // Epilogue teams: three teams of four warps (448 threads at <= 72 registers) by default -- the
-  // epilogues are bound by MUFU / dependent-issue latency, not bytes, and 50 % more warps hide it
-  // (measured on the D0 step: 4.68 ms with two teams, 4.53 ms with three, all layers);
+  // Consumer warpgroups: two by default (one in its epilogue while the other one's MMAs run);
   // edet_set_option("pw_teams", 2 | 3) forces a variant for A/B measurements.
   const int opt_teams = option_pw_teams();
-  const int teams = am ? 3 : (opt_teams ? opt_teams : 3);
-  const int epi_warps = 4 * teams, slab_bytes = teams == 2 ? 4096 : 2048;
-  p.block_n = pick_block_n(nout, teams);
+  const int teams = opt_teams ? opt_teams : 2;
+  p.block_n = am ? kArgmaxCols : pick_block_n(nout);
   p.num_m_blocks = ceil_div(rows, BLOCK_M);
   p.num_n_blocks = ceil_div(nout, p.block_n);
-  // k-block / smem row pitch: 16 halves (32B swizzle) for K <= 16, 32 (64B) for K <= 32, else
-  // 64 (128B) -- unless two 64-wide stages of this (wide) N tile would not fit next to the store
-  // slabs, in which case the narrower 32-wide stages keep the pipeline >= 3 deep.
   p.wbatch = wbatch;
   p.ldr = ldr;
   p.bias = bias;
   p.residual = residual;
-  // accumulator stages: as many as fit in this CTA's 256 TMEM columns (two CTAs per SM), up to 4
-  // with three teams (so that every team can work on its own tile of a thin layer), 2 with two
-  p.accum_stages = 256 / p.block_n;
-  if (p.accum_stages < 1) p.accum_stages = 1;
-  if (p.accum_stages > (teams == 3 ? kMaxAccum : 2)) p.accum_stages = teams == 3 ? kMaxAccum : 2;
-  int cols = 32;
-  while (cols < p.accum_stages * p.block_n) cols *= 2;
-  p.tmem_cols = cols;
   p.total_tiles = batch * p.num_m_blocks * p.num_n_blocks;
   p.sched = next_sched_slot();
   if (!p.sched) return EDET_ERR_CUDA;
 
-  // k-block / smem row pitch: 16 halves (32B swizzle) for K <= 16, 32 (64B) for K <= 32, else 64
-  // (128B).  Two store slabs per epilogue warp when they fit; a wide N tile falls back first to
-  // one slab, then to 32-wide k-blocks, so that the TMA ring stays >= 3 deep (>= 2 at worst).
   // every column the epilogue can touch: whole N tiles (n_valid is rounded up to 16 inside a tile)
   const int bias_cols = p.num_n_blocks * p.block_n;
   EDET_CHECK_ARG(bias_cols <= kMaxBiasSmem, "pointwise_tc: nout %d too wide", nout);
   p.bias_floats = bias_cols;
-  const int ctrl = p.bias_floats * 4 + (2 * kMaxStages + 2 * kMaxAccum + 2 * kRing) * 8 + 16 + 16 * kRing;
-  int best_stages = 0, fixed = 0, stage_bytes = 0;
-  auto plan = [&](int limit) {
-    best_stages = 0;
-    for (int attempt = 0; attempt < 4 && best_stages < 3; ++attempt) {
-      const int bk = k <= 16 ? 16 : (k <= 32 ? 32 : (attempt >= 2 ? 32 : 64));
-      const int slabs = (attempt & 1) ? 1 : 2;
-      const int a_bytes = BLOCK_M * bk * 2;
-      const int b_bytes = ((p.block_n * bk * 2 + 1023) / 1024) * 1024;
-      const int fx = slabs * epi_warps * slab_bytes + ctrl;
-      int st = (limit - 1024 - fx) / (a_bytes + b_bytes);
-      if (st > kMaxStages) st = kMaxStages;
-      if (st > best_stages) {
-        best_stages = st;
-        p.block_k = bk;
-        p.slabs_per_warp = slabs;
-        p.a_stage_bytes = a_bytes;
-        p.b_stage_bytes = b_bytes;
-        fixed = fx;
-        stage_bytes = a_bytes + b_bytes;
-      }
-    }
-  };
-  // Shared-memory budget.  The NMS of the previous batch (one 126 KiB CTA per image, own stream)
-  // runs under the first layers of the next network: with 99 KiB a pointwise CTA fits next to it
-  // (99 + 126 + 2 KiB <= 228 KiB), with 113 KiB those SMs stay empty.  So 99 KiB wherever that
-  // still gives a ring of >= 4 stages (every thin-K layer), the full half SM otherwise.
+  // k-block / smem row pitch: 16 halves (32B swizzle) for K <= 16, 32 (64B) for K <= 32, else 64
+  // (128B), so that a stage only holds bytes that exist.
+  p.block_k = k <= 16 ? 16 : (k <= 32 ? 32 : 64);
+  p.a_stage_bytes = BLOCK_M * p.block_k * 2;
+  p.b_stage_bytes = ((p.block_n * p.block_k * 2 + 1023) / 1024) * 1024;
+  const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
+  const int fixed = teams * kSlabsPerTeam * kSlabBytes + p.bias_floats * 4 +
+                    (2 * kMaxStages + 2 * kRing) * 8 + 16 * kRing;
   const int opt_kb = option_pw_smem_kb();
-  if (opt_kb) {
-    plan(opt_kb * 1024);
-  } else {
-    plan(kSmemCoResident);
-    if (best_stages < 4) plan(kSmemLimit);
-  }
-  EDET_CHECK_ARG(best_stages >= 2, "pointwise_tc: block_n %d leaves <2 pipeline stages", p.block_n);
-  p.num_stages = best_stages;
-  p.desc_layout = p.block_k == 64 ? 2 : (p.block_k == 32 ? 4 : 6);
+  const int limit = opt_kb ? opt_kb * 1024 : kSmemLimit;
+  int stages = (limit - 1024 - fixed) / stage_bytes;
+  if (stages > kMaxStages) stages = kMaxStages;
+  p.team_stages = stages / teams;            // each consumer's own ring
+  EDET_CHECK_ARG(p.team_stages >= 2, "pointwise_tc: block_n %d leaves <2 pipeline stages per consumer",
+                 p.block_n);
+  stages = p.team_stages * teams;
+  p.num_stages = stages;
+  p.desc_layout = desc_layout_for(p.block_k);
   p.desc_sbo = 8 * p.block_k * 2;
   p.num_k_blocks = ceil_div(k, p.block_k);
-  const int smem_bytes = 1024 + best_stages * stage_bytes + fixed;
+  const int smem_bytes = 1024 + stages * stage_bytes + fixed;
 
   CUtensorMap ma, mw, mo;
   int rc;
@@ -718,21 +430,21 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   if ((rc = make_map(&mw, wt, k, nout, wbatch, k, static_cast<uint64_t>(nout) * k, p.block_n,
                      p.block_k)))
     return rc;
-  // store box: [32 rows] x 64 columns (128B swizzle) for two teams, x 32 columns (64B) for three
+  // store box: [64 rows] x 64 columns, 128B swizzle
   if (am) {
     mo = mw;   // the arg-max epilogue stores nothing through TMA
-  } else if ((rc = make_map(&mo, out, nout, rows, batch, ldo, static_cast<uint64_t>(rows) * ldo, 32,
-                            teams == 2 ? 64 : 32))) {
+  } else if ((rc = make_map(&mo, out, nout, rows, batch, ldo, static_cast<uint64_t>(rows) * ldo,
+                            BLOCK_M, kStoreCols))) {
     return rc;
   }
 
   const int sm_count = device_sm_count();
   if (!sm_count) return EDET_ERR_CUDA;
-  int grid = 2 * sm_count - option_persist_slack();
-  if (grid < sm_count) grid = sm_count;
+  int grid = sm_count - option_persist_slack();
+  if (grid < 1) grid = 1;
   if (p.total_tiles < grid) grid = p.total_tiles;
   const bool has_res = residual != nullptr;
-  if (am) return launch<EDET_ACT_NONE, false, 3, EPI_ARGMAX>(ma, mw, mo, p, grid, smem_bytes, stream);
+  if (am) return launch<EDET_ACT_NONE, false, 2, EPI_ARGMAX>(ma, mw, mo, p, grid, smem_bytes, stream);
 
 #define EDET_PW_CASE(A)                                                                       \
   if (teams == 3)                                                                             \

@@ -1,16 +1,17 @@
 // Separable convolution of a head tower layer as ONE kernel:
 //   depthwise 3x3 'SAME'  ->  pointwise 1x1 on the tensor cores (+ bias, BN folded) (+ act)
 // The depthwise result never reaches HBM: it is written as fp16 straight into the 128B-swizzled
-// K-major shared-memory tile that tcgen05.mma reads as its A operand.
+// K-major shared-memory tile that wgmma reads as its A operand.
 //
 // Replaces, per tower layer, efficientdet_arch.py:149-191 / 206-249 (SeparableConv2D, per-level
 // BN, activation).  Algorithmic HBM bytes per launch: 2*N*h*w*(c + nout) + weights -- the
 // [N,h,w,c] depthwise output (written and read back by a depthwise + pointwise pair) is gone.
 //
-// One CTA = one 8x16 output tile (128 pixels = the M of one UMMA), persistent over tiles:
+// One CTA (one warpgroup) = one 8x16 output tile (128 pixels), persistent over tiles:
 //   1. all warps: depthwise 3x3 -> fp16 A tile [128 px][c] (swizzled K-major atoms)
-//   2. one thread: tcgen05.mma  D[128 px][nout] = A * W^T  (W loaded once per CTA by TMA)
-//   3. all warps: TMEM -> +bias, act -> fp16 -> global (32 contiguous bytes per tcgen05.ld)
+//   2. the warpgroup, per 64-pixel half: wgmma  D[64 px][nout] = A * W^T into registers
+//      (W loaded once per CTA by TMA)
+//   3. every thread: its accumulator fragment -> +bias, act -> fp16 -> global
 //
 // The whole-BiFPN-node form of this kernel (resample + weighted fusion + activation in front of
 // the depthwise) was removed in round 2: measured on the D0 step it was slower than the
@@ -36,7 +37,7 @@ struct Params {
   const float* bias;      // [nout]
   __half* out;            // [n, h, w, ldo]
   int n, h, w, c, nout, ldo;
-  int katoms, kpad, npad, b_atom_bytes, tmem_cols;
+  int katoms, kpad, npad, b_atom_bytes;
   int tiles_x, tiles_y, total_tiles;
   unsigned* sched;        // dynamic tile scheduler slot (direct kernel)
 };
@@ -44,9 +45,54 @@ struct Params {
 // ---- single-input form (head tower layers): depthwise straight from global memory ------------
 // No fusion and no pre-activation, so the input tile needs no staging: each thread owns one
 // channel pair x 4 columns x the 8 rows of the tile (the register tiling of depthwise.cu: fp32
-// weights in registers, packed FFMA2, loads software-pipelined two rows ahead), and drops its 32
+// weights in registers, FFMA on channel pairs, loads software-pipelined two rows ahead), and drops its 32
 // fp16 pairs into the swizzled A tile.  128 threads per CTA, up to 4 CTAs per SM.
 constexpr int kDirectThreads = 128;
+
+// Steps 2 + 3 of both kernels: D = A * W^T for the two 64-pixel halves of the tile in turn (64
+// accumulator registers per thread), each followed by its epilogue straight from the fragments.
+// A: katoms atoms of [128 px][64] halves (128B swizzle), B: katoms atoms of [npad][64].
+template <int ACT_POST>
+__device__ __forceinline__ void mma_epilogue(const Params& p, uint32_t a_u32, uint32_t b_u32,
+                                             int katoms, int n, int y0, int x0) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nt = p.npad >> 4;
+  const int cq = 2 * (lane & 3);
+#pragma unroll 1
+  for (int mb = 0; mb < 2; ++mb) {
+    float acc[kMaxN / 16][8] = {};
+    wg_fence();
+    for (int kb = 0; kb < katoms; ++kb) {
+      const uint64_t da = make_smem_desc(a_u32 + kb * kAtomBytesA + mb * 64 * 128, 1024, 1);
+      const uint64_t db = make_smem_desc(b_u32 + kb * p.b_atom_bytes, 1024, 1);
+      wg_mma_kblock<kMaxN / 16>(acc, da, db, 128, nt, min(4, (p.kpad - kb * 64) >> 4), kb == 0);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc<kMaxN / 16>(acc);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = mb * 64 + 16 * warp + (lane >> 2) + 8 * r;
+      const int y = y0 + row / TW, x = x0 + row % TW;
+      if (y >= p.h || x >= p.w) continue;
+      __half* orow = p.out + ((static_cast<size_t>(n) * p.h + y) * p.w + x) * p.ldo;
+#pragma unroll
+      for (int j = 0; j < kMaxN / 16; ++j) {
+        const int col = 16 * j + cq;
+        if (col >= p.nout) continue;
+        const bool hi_ok = col + 8 < p.nout;
+        const float2 b_lo = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+        const float2 b_hi = hi_ok ? __ldg(reinterpret_cast<const float2*>(p.bias + col + 8))
+                                  : make_float2(0.f, 0.f);
+        float2 lo = fadd2_rn(make_float2(acc[j][2 * r], acc[j][2 * r + 1]), b_lo);
+        float2 hi = fadd2_rn(make_float2(acc[j][4 + 2 * r], acc[j][4 + 2 * r + 1]), b_hi);
+        if (ACT_POST != EDET_ACT_NONE) apply_act4<ACT_POST>(lo, hi);
+        *reinterpret_cast<__half2*>(orow + col) = __floats2half2_rn(lo.x, lo.y);
+        if (hi_ok) *reinterpret_cast<__half2*>(orow + col + 8) = __floats2half2_rn(hi.x, hi.y);
+      }
+    }
+  }
+}
 
 template <int ACT_POST>
 __global__ void __launch_bounds__(kDirectThreads, 4)
@@ -60,31 +106,16 @@ sepconv_direct_kernel(const __grid_constant__ CUtensorMap map_w, const Params p)
   uint8_t* smem_b = smem_a + p.katoms * kAtomBytesA;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + p.katoms * p.b_atom_bytes);
   const uint32_t w_bar = smem_u32(bars);
-  const uint32_t mma_bar = smem_u32(bars + 1);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     mbar_init(w_bar, 1);
-    mbar_init(mma_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
-  }
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   // the K-padding channels of A multiply TMA-zero-filled weights: they must be finite -> zero A once
   for (int i = threadIdx.x; i < p.katoms * kAtomBytesA / 16; i += kDirectThreads)
     reinterpret_cast<uint4*>(smem_a)[i] = make_uint4(0u, 0u, 0u, 0u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (threadIdx.x == 0) {
     mbar_expect_tx(w_bar, static_cast<uint32_t>(p.katoms * p.npad * 128));
     for (int kb = 0; kb < p.katoms; ++kb)
@@ -97,10 +128,7 @@ sepconv_direct_kernel(const __grid_constant__ CUtensorMap map_w, const Params p)
   const float2* w2 = reinterpret_cast<const float2*>(p.dw_w);
   pdl_wait_prior();
 
-  const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(p.npad >> 3) << 17) |
-                         (static_cast<uint32_t>(BLOCK_M >> 4) << 24);
   const uint32_t a_u32 = smem_u32(smem_a);
-  uint32_t mma_phase = 0;
   bool weights_ready = false;
 
   __shared__ int next_tile_s[2];   // double buffered: slot (it & 1) is rewritten two iterations later
@@ -156,7 +184,7 @@ sepconv_direct_kernel(const __grid_constant__ CUtensorMap map_w, const Params p)
               for (int j = 0; j < 4; ++j)
 #pragma unroll
                 for (int kx = 0; kx < 3; ++kx)
-                  acc[r][j] = __ffma2_rn(xv[j + kx], wreg[ky * 3 + kx], acc[r][j]);
+                  acc[r][j] = ffma2_rn(xv[j + kx], wreg[ky * 3 + kx], acc[r][j]);
             }
           }
         }
@@ -185,7 +213,7 @@ sepconv_direct_kernel(const __grid_constant__ CUtensorMap map_w, const Params p)
               for (int j = 0; j < 4; ++j)
 #pragma unroll
                 for (int kx = 0; kx < 3; ++kx)
-                  acc[r][j] = __ffma2_rn(xv[j + kx], wreg[ky * 3 + kx], acc[r][j]);
+                  acc[r][j] = ffma2_rn(xv[j + kx], wreg[ky * 3 + kx], acc[r][j]);
             }
           }
         }
@@ -206,74 +234,17 @@ sepconv_direct_kernel(const __grid_constant__ CUtensorMap map_w, const Params p)
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    // ---- D = A * W^T ---------------------------------------------------------------------------
-    if (threadIdx.x == 0) {
-      if (!weights_ready) {
-        mbar_wait(w_bar, 0);
-        weights_ready = true;
-      }
-      tc_fence_after();
-      for (int kb = 0; kb < p.katoms; ++kb) {
-        const uint64_t da = make_smem_desc(a_u32 + kb * kAtomBytesA, 1024, 2);
-        const uint64_t db = make_smem_desc(smem_u32(smem_b + kb * p.b_atom_bytes), 1024, 2);
-        const int ksteps = min(4, (p.kpad - kb * 64) >> 4);
-        for (int ks = 0; ks < ksteps; ++ks)
-          tc_mma_f16(tmem_base, da + static_cast<uint64_t>(ks * 2), db + static_cast<uint64_t>(ks * 2),
-                     idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-      }
-      tc_commit(mma_bar);
+    if (!weights_ready) {
+      mbar_wait(w_bar, 0);
+      weights_ready = true;
     }
-    mbar_wait(mma_bar, mma_phase);
-    mma_phase ^= 1;
-    tc_fence_after();
-    // ---- epilogue: warp w owns TMEM lanes (= tile rows) 32w .. 32w+31, all columns ---------------
-    {
-      const int row = warp * 32 + lane;
-      const int y = y0 + row / TW, x = x0 + row % TW;
-      const bool ok = y < h && x < wd;
-      __half* orow = p.out + ((static_cast<size_t>(n) * h + y) * wd + x) * p.ldo;
-      for (int col = 0; col < p.npad; col += 16) {
-        float v[16];
-        tc_ld16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + static_cast<uint32_t>(col), v);
-        tc_wait_ld();
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int cc = col + hh * 8;
-          if (ok && cc < p.nout) {
-            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + cc));
-            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + cc + 4));
-            float2 r0 = __fadd2_rn(make_float2(v[hh * 8 + 0], v[hh * 8 + 1]), make_float2(b0.x, b0.y));
-            float2 r1 = __fadd2_rn(make_float2(v[hh * 8 + 2], v[hh * 8 + 3]), make_float2(b0.z, b0.w));
-            float2 r2 = __fadd2_rn(make_float2(v[hh * 8 + 4], v[hh * 8 + 5]), make_float2(b1.x, b1.y));
-            float2 r3 = __fadd2_rn(make_float2(v[hh * 8 + 6], v[hh * 8 + 7]), make_float2(b1.z, b1.w));
-            if (ACT_POST != EDET_ACT_NONE) {
-              apply_act4<ACT_POST>(r0, r1);
-              apply_act4<ACT_POST>(r2, r3);
-            }
-            const float o[8] = {r0.x, r0.y, r1.x, r1.y, r2.x, r2.y, r3.x, r3.y};
-            *reinterpret_cast<uint4*>(orow + cc) = float_to_half8(o);
-          }
-        }
-      }
-    }
-    tc_fence_before();
+    mma_epilogue<ACT_POST>(p, a_u32, smem_u32(smem_b), p.katoms, n, y0, x0);
     __syncthreads();
-    tc_fence_after();
     t = next_tile_s[it & 1];
   }
 
   if (threadIdx.x == 0 && !weights_ready) mbar_wait(w_bar, 0);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-  }
 }
 
 // ---- single-input form, c <= 64, input tile staged by TMA --------------------------------------
@@ -302,37 +273,22 @@ sepconv_direct_tma_kernel(const __grid_constant__ CUtensorMap map_w,
   uint8_t* smem_in = smem_b + p.b_atom_bytes;              // 2 x [HT][WT][64] halves, dense
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_in + NBUF * kInTileBytes);
   const uint32_t w_bar = smem_u32(bars);
-  const uint32_t mma_bar = smem_u32(bars + 1);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
   // [2] x {tile, image, tile row, tile column}: thread 0 decodes the next tile (its divisions)
   // when it fetches it; everybody reads the coordinates with one 16-byte load
-  volatile int4* next_tile_s = reinterpret_cast<volatile int4*>(tmem_slot + 4);
+  volatile int4* next_tile_s = reinterpret_cast<volatile int4*>(bars + 4);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     mbar_init(w_bar, 1);
-    mbar_init(mma_bar, 1);
     mbar_init(smem_u32(bars + 2), 1);
     mbar_init(smem_u32(bars + 3), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
   }
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   // the K-padding channels of A multiply TMA-zero-filled weights: they must be finite -> zero A once
   for (int i = threadIdx.x; i < kAtomBytesA / 16; i += kDirectThreads)
     reinterpret_cast<uint4*>(smem_a)[i] = make_uint4(0u, 0u, 0u, 0u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (threadIdx.x == 0) {
     mbar_expect_tx(w_bar, static_cast<uint32_t>(p.npad * 128));
     tma_load_3d(smem_u32(smem_b), &map_w, w_bar, 0, 0, 0);
@@ -355,10 +311,7 @@ sepconv_direct_tma_kernel(const __grid_constant__ CUtensorMap map_w,
     tma_load_4d(smem_u32(smem_in + slot * kInTileBytes), &map_x, bar, 0, tc.w * TW - 1, tc.z * TH - 1, tc.y);
   };
 
-  const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(p.npad >> 3) << 17) |
-                         (static_cast<uint32_t>(BLOCK_M >> 4) << 24);
   const uint32_t a_u32 = smem_u32(smem_a);
-  uint32_t mma_phase = 0;
   bool weights_ready = false;
 
   int4 cur = decode(blockIdx.x);
@@ -404,7 +357,7 @@ sepconv_direct_tma_kernel(const __grid_constant__ CUtensorMap map_w,
             for (int j = 0; j < 4; ++j)
 #pragma unroll
               for (int kx = 0; kx < 3; ++kx)
-                acc[r][j] = __ffma2_rn(xv[j + kx], wreg[ky * 3 + kx], acc[r][j]);
+                acc[r][j] = ffma2_rn(xv[j + kx], wreg[ky * 3 + kx], acc[r][j]);
           }
         }
       }
@@ -424,76 +377,21 @@ sepconv_direct_tma_kernel(const __grid_constant__ CUtensorMap map_w,
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
     if (NBUF == 1 && threadIdx.x == 0) {       // the input buffer is free again: prefetch the next tile
       const int4 nx = const_cast<const int4*>(next_tile_s)[it & 1];
       if (nx.x < p.total_tiles) fetch_tile(nx, 0);
     }
-    // ---- D = A * W^T ---------------------------------------------------------------------------
-    if (threadIdx.x == 0) {
-      if (!weights_ready) {
-        mbar_wait(w_bar, 0);
-        weights_ready = true;
-      }
-      tc_fence_after();
-      const uint64_t da = make_smem_desc(a_u32, 1024, 2);
-      const uint64_t db = make_smem_desc(smem_u32(smem_b), 1024, 2);
-      const int ksteps = min(4, p.kpad >> 4);
-      for (int ks = 0; ks < ksteps; ++ks)
-        tc_mma_f16(tmem_base, da + static_cast<uint64_t>(ks * 2), db + static_cast<uint64_t>(ks * 2),
-                   idesc, ks > 0 ? 1u : 0u);
-      tc_commit(mma_bar);
+    if (!weights_ready) {
+      mbar_wait(w_bar, 0);
+      weights_ready = true;
     }
-    mbar_wait(mma_bar, mma_phase);
-    mma_phase ^= 1;
-    tc_fence_after();
-    // ---- epilogue: warp w owns TMEM lanes (= tile rows) 32w .. 32w+31, all columns ---------------
-    {
-      const int row = warp * 32 + lane;
-      const int y = y0 + row / TW, x = x0 + row % TW;
-      const bool ok = y < h && x < wd;
-      __half* orow = p.out + ((static_cast<size_t>(n) * h + y) * wd + x) * p.ldo;
-      for (int col = 0; col < p.npad; col += 16) {
-        float v[16];
-        tc_ld16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + static_cast<uint32_t>(col), v);
-        tc_wait_ld();
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int cc = col + hh * 8;
-          if (ok && cc < p.nout) {
-            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + cc));
-            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + cc + 4));
-            float2 r0 = __fadd2_rn(make_float2(v[hh * 8 + 0], v[hh * 8 + 1]), make_float2(b0.x, b0.y));
-            float2 r1 = __fadd2_rn(make_float2(v[hh * 8 + 2], v[hh * 8 + 3]), make_float2(b0.z, b0.w));
-            float2 r2 = __fadd2_rn(make_float2(v[hh * 8 + 4], v[hh * 8 + 5]), make_float2(b1.x, b1.y));
-            float2 r3 = __fadd2_rn(make_float2(v[hh * 8 + 6], v[hh * 8 + 7]), make_float2(b1.z, b1.w));
-            if (ACT_POST != EDET_ACT_NONE) {
-              apply_act4<ACT_POST>(r0, r1);
-              apply_act4<ACT_POST>(r2, r3);
-            }
-            const float o[8] = {r0.x, r0.y, r1.x, r1.y, r2.x, r2.y, r3.x, r3.y};
-            *reinterpret_cast<uint4*>(orow + cc) = float_to_half8(o);
-          }
-        }
-      }
-    }
-    tc_fence_before();
+    mma_epilogue<ACT_POST>(p, a_u32, smem_u32(smem_b), 1, n, y0, x0);
     __syncthreads();
-    tc_fence_after();
     cur = const_cast<const int4*>(next_tile_s)[it & 1];
   }
 
   if (threadIdx.x == 0 && !weights_ready) mbar_wait(w_bar, 0);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-  }
 }
 
 template <int POST, int NBUF>
@@ -541,9 +439,6 @@ extern "C" int edet_sepconv(const edet_fuse_input* h_inputs, int n_inputs, int p
   p.kpad = ((c + 15) / 16) * 16;
   p.npad = ((nout + 15) / 16) * 16;
   p.b_atom_bytes = ((p.npad * 128 + 1023) / 1024) * 1024;
-  int cols = 32;
-  while (cols < p.npad) cols *= 2;
-  p.tmem_cols = cols;
   p.tiles_x = ceil_div(wd, TW); p.tiles_y = ceil_div(h, TH);
   p.total_tiles = n * p.tiles_x * p.tiles_y;
   CUtensorMap mw;
@@ -558,7 +453,6 @@ extern "C" int edet_sepconv(const edet_fuse_input* h_inputs, int n_inputs, int p
                       p.fuse.in[0].weight == 1.0f && pre_act == EDET_ACT_NONE;
   const int smem_bytes = 1024 + p.katoms * (kAtomBytesA + p.b_atom_bytes) + 64;
   int per_sm = 232448 / (smem_bytes + 1024);
-  if (per_sm * p.tmem_cols > 512) per_sm = 512 / p.tmem_cols;
   const int cap = 4;
   if (per_sm > cap) per_sm = cap;
   if (per_sm < 1) per_sm = 1;
@@ -571,7 +465,6 @@ extern "C" int edet_sepconv(const edet_fuse_input* h_inputs, int n_inputs, int p
     const int nbuf = option_sepconv_impl() == 2 ? 2 : 1;
     const int smem_tma = 1024 + kAtomBytesA + p.b_atom_bytes + nbuf * kInTileBytes + 128;
     int per = 232448 / (smem_tma + 1024);
-    if (per * p.tmem_cols > 512) per = 512 / p.tmem_cols;
     if (per > (nbuf == 1 ? 4 : 3)) per = nbuf == 1 ? 4 : 3;
     const int grid_tma = p.total_tiles < per * sm_count ? p.total_tiles : per * sm_count;
 #define EDET_SEPC_TMA(POST)                                                                   \

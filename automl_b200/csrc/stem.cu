@@ -1,7 +1,7 @@
 // Stem: Conv2D 3x3 stride 2 'SAME', 3 -> cout (24..64), + folded BN + activation.
 // Reads the float32 NHWC image the reference feeds the network (efficientnet_model.py:526-527)
 // and writes NHWC fp16.  bytes = 12*n*h*w + 2*n*ho*wo*cout; 27 MACs per output element, so the
-// arithmetic runs on the packed fp32 pipe (FFMA2) to stay under the HBM time.
+// arithmetic runs as fp32 FMAs on channel pairs.
 //
 // One thread = two horizontally adjacent output pixels x 16 output channels (8 channel pairs);
 // the [27][16] weight slab of the channel half sits in shared memory as float2 pairs and is read
@@ -72,10 +72,10 @@ stem_kernel(const float* __restrict__ in, __half* __restrict__ out, const __half
           for (int q = 0; q < kStemCh / 4; ++q) {
             const float4 w4 = *reinterpret_cast<const float4*>(&ws[t][2 * q]);
             const float2 wa = make_float2(w4.x, w4.y), wb = make_float2(w4.z, w4.w);
-            acc0[2 * q] = __ffma2_rn(a0, wa, acc0[2 * q]);
-            acc0[2 * q + 1] = __ffma2_rn(a0, wb, acc0[2 * q + 1]);
-            acc1[2 * q] = __ffma2_rn(a1, wa, acc1[2 * q]);
-            acc1[2 * q + 1] = __ffma2_rn(a1, wb, acc1[2 * q + 1]);
+            acc0[2 * q] = ffma2_rn(a0, wa, acc0[2 * q]);
+            acc0[2 * q + 1] = ffma2_rn(a0, wb, acc0[2 * q + 1]);
+            acc1[2 * q] = ffma2_rn(a1, wa, acc1[2 * q]);
+            acc1[2 * q + 1] = ffma2_rn(a1, wb, acc1[2 * q + 1]);
           }
         }
       }

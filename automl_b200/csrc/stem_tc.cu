@@ -5,19 +5,19 @@
 // 526-527).  To keep its precision on the fp16 tensor-core path every input value is split into
 // two fp16 terms, x = hi + lo (hi = fp16(x), lo = fp16(x - hi): ~22 significant bits), and the 27
 // taps become K = 54 (padded to 64 = one 128-byte swizzled K atom): columns 0..26 hold hi, 27..53
-// hold lo, and W' repeats the 27 fp16 weights for both halves.  fp32 accumulation in TMEM.
+// hold lo, and W' repeats the 27 fp16 weights for both halves.  fp32 accumulation in registers.
 // The 27-MAC-per-output CUDA-core kernel (stem.cu) was FFMA-issue bound at 0.21 of the HBM
-// roofline; here the arithmetic is 4 tcgen05.mma per tile and the CUDA cores only build the A
+// roofline; here the arithmetic is 2 x 4 wgmma per tile and the CUDA cores only build the A
 // tile (27 loads + 27 splits per pixel) and run the epilogue.
 //
-// One CTA (128 threads, one thread per output pixel of the tile) per tile, persistent with the
-// dynamic tile scheduler, 5 CTAs per SM:
+// One CTA (128 threads = one warpgroup, one thread per output pixel of the tile when the A tile
+// is built) per tile, persistent with the dynamic tile scheduler, up to 4 CTAs per SM:
 //   1. all threads: the (17 x 33 x 3) float32 input patch -> shared memory with cp.async (coalesced,
 //      zero filled outside the image = 'SAME' padding), double buffered: the NEXT tile's patch is
 //      in flight while this tile is converted, multiplied and written out
 //   2. thread m: its 27 inputs -> hi / lo halves -> row m of the swizzled A tile
-//   3. one thread: 4 x tcgen05.mma (M 128, N cout rounded to 16, K 16)
-//   4. warp w: TMEM lanes 32w.. -> + bias -> activation -> fp16 -> global
+//   3. the warpgroup: wgmma (two M 64 halves, N cout rounded to 16, K 16) into registers
+//   4. every thread: its accumulator fragment -> + bias -> activation -> fp16 -> global
 // Bytes per launch (SURVEY.md 8d): 12*n*h*w + 2*n*ho*wo*cout.
 #include "tc_common.cuh"
 
@@ -27,7 +27,7 @@ namespace stemtc {
 using namespace pwtc;
 
 constexpr int kThreads = 128;
-constexpr int TH = 8, TW = 16;                       // output tile: 128 pixels = the M of one UMMA
+constexpr int TH = 8, TW = 16;                       // output tile: 128 pixels = two wgmma M blocks
 constexpr int IH = 2 * TH + 1, IW = 2 * TW + 1;      // input patch (stride 2, 3 x 3 window)
 constexpr int kRowFloats = IW * 3;                   // 99 floats per patch row
 constexpr int kInFloats = IH * kRowFloats;           // 1683
@@ -56,12 +56,12 @@ struct Params {
   const __half* wgt;    // [27][cout]  (ky, kx, cin major; BN scale folded)
   const float* bias;    // [cout]
   int n, h, w, ho, wo, cout, npad, pad_t, pad_l;
-  int tiles_x, tiles_y, total_tiles, tmem_cols;
+  int tiles_x, tiles_y, total_tiles;
   unsigned* sched;
 };
 
 template <int ACT>
-__global__ void __launch_bounds__(kThreads, 6)
+__global__ void __launch_bounds__(kThreads, 4)
 stem_tc_kernel(const Params p) {
   pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -70,27 +70,11 @@ stem_tc_kernel(const Params p) {
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem_a + kABytes;
   float* in_s = reinterpret_cast<float*>(smem_b + kBBytes);                 // [2][IH][IW][3]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(in_s + 2 * kInPad);
-  const uint32_t mma_bar = smem_u32(bars);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 1);
   // [2] x {tile, image, tile row, tile column}: thread 0 decodes the next tile once (the integer
   // divisions); everybody reads the coordinates with one 16-byte load
-  volatile int4* next_tile_s = reinterpret_cast<volatile int4*>(
-      (reinterpret_cast<uintptr_t>(tmem_slot + 2) + 15) & ~static_cast<uintptr_t>(15));
+  volatile int4* next_tile_s = reinterpret_cast<volatile int4*>(in_s + 2 * kInPad);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(mma_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   // W' tile [npad][64] (K-major, 128B swizzle): k < 27 -> w[k], 27 <= k < 54 -> w[k - 27], else 0;
   // rows >= cout are zero.  Constants: built before the PDL wait.
   for (int i = threadIdx.x; i < p.npad * 64; i += kThreads) {
@@ -100,17 +84,12 @@ stem_tc_kernel(const Params p) {
     *reinterpret_cast<__half*>(smem_b + nrow * 128 + ((((k >> 3) ^ (nrow & 7))) << 4) + (k & 7) * 2) = v;
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait_prior();
 
-  const uint32_t idesc = (1u << 4) | (static_cast<uint32_t>(p.npad >> 3) << 17) |
-                         (static_cast<uint32_t>(BLOCK_M >> 4) << 24);
   const uint32_t a_u32 = smem_u32(smem_a);
   const uint32_t in_u32 = smem_u32(in_s);
-  uint32_t mma_phase = 0;
+  const int nt = p.npad >> 4;
   const int m = threadIdx.x;                         // this thread's pixel of the tile
   const int mr = m / TW, mc = m % TW;
   const int row_floats = p.w * 3;
@@ -186,63 +165,48 @@ stem_tc_kernel(const Params p) {
       }
     }
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    // ---- 3. D = A * W'^T -------------------------------------------------------------------------
-    if (threadIdx.x == 0) {
-      tc_fence_after();
-      const uint64_t da = make_smem_desc(a_u32, 1024, 2);
-      const uint64_t db = make_smem_desc(smem_u32(smem_b), 1024, 2);
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
-        tc_mma_f16(tmem_base, da + static_cast<uint64_t>(ks * 2), db + static_cast<uint64_t>(ks * 2),
-                   idesc, ks > 0 ? 1u : 0u);
-      tc_commit(mma_bar);
-    }
-    mbar_wait(mma_bar, mma_phase);
-    mma_phase ^= 1;
-    tc_fence_after();
-    // ---- 4. epilogue: thread m owns TMEM lane m = its pixel --------------------------------------
+    // ---- 3. D = A * W'^T: rows 64 mb .. 64 mb + 63 into acc[mb] -----------------------------------
+    float acc[2][kMaxN / 16][8] = {};
     {
-      const int y = y0 + mr, x = x0 + mc;
-      const bool ok = y < p.ho && x < p.wo;
-      __half* orow = p.out + ((static_cast<size_t>(n) * p.ho + y) * p.wo + x) * p.cout;
-      for (int col = 0; col < p.npad; col += 16) {
-        float v[16];
-        tc_ld16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + static_cast<uint32_t>(col), v);
-        tc_wait_ld();
+      const uint64_t db = make_smem_desc(smem_u32(smem_b), 1024, 1);
+      wg_fence();
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int cc = col + hh * 8;
-          if (ok && cc < p.cout) {
-            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + cc));
-            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + cc + 4));
-            float2 r0 = __fadd2_rn(make_float2(v[hh * 8 + 0], v[hh * 8 + 1]), make_float2(b0.x, b0.y));
-            float2 r1 = __fadd2_rn(make_float2(v[hh * 8 + 2], v[hh * 8 + 3]), make_float2(b0.z, b0.w));
-            float2 r2 = __fadd2_rn(make_float2(v[hh * 8 + 4], v[hh * 8 + 5]), make_float2(b1.x, b1.y));
-            float2 r3 = __fadd2_rn(make_float2(v[hh * 8 + 6], v[hh * 8 + 7]), make_float2(b1.z, b1.w));
-            apply_act4<ACT>(r0, r1);
-            apply_act4<ACT>(r2, r3);
-            const float o[8] = {r0.x, r0.y, r1.x, r1.y, r2.x, r2.y, r3.x, r3.y};
-            *reinterpret_cast<uint4*>(orow + cc) = float_to_half8(o);
-          }
+      for (int mb = 0; mb < 2; ++mb)
+        wg_mma_kblock<kMaxN / 16>(acc[mb], make_smem_desc(a_u32 + mb * 64 * 128, 1024, 1), db, 128,
+                                  nt, 4, true);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc<kMaxN / 16>(acc[0]);
+      wg_fence_acc<kMaxN / 16>(acc[1]);
+    }
+    // ---- 4. epilogue from the accumulator fragments: rows r0, r0 + 8 of each M block ------------
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int row = mb * 64 + 16 * warp + (lane >> 2) + 8 * r;
+        const int y = y0 + row / TW, x = x0 + row % TW;
+        if (y >= p.ho || x >= p.wo) continue;
+        __half* orow = p.out + ((static_cast<size_t>(n) * p.ho + y) * p.wo + x) * p.cout;
+#pragma unroll
+        for (int j = 0; j < kMaxN / 16; ++j) {
+          const int col = 16 * j + 2 * (lane & 3);
+          if (col >= p.cout) continue;
+          const bool hi_ok = col + 8 < p.cout;
+          const float2 b_lo = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+          const float2 b_hi = hi_ok ? __ldg(reinterpret_cast<const float2*>(p.bias + col + 8))
+                                    : make_float2(0.f, 0.f);
+          float2 lo = fadd2_rn(make_float2(acc[mb][j][2 * r], acc[mb][j][2 * r + 1]), b_lo);
+          float2 hi = fadd2_rn(make_float2(acc[mb][j][4 + 2 * r], acc[mb][j][4 + 2 * r + 1]), b_hi);
+          apply_act4<ACT>(lo, hi);
+          *reinterpret_cast<__half2*>(orow + col) = __floats2half2_rn(lo.x, lo.y);
+          if (hi_ok) *reinterpret_cast<__half2*>(orow + col + 8) = __floats2half2_rn(hi.x, hi.y);
         }
       }
     }
-    tc_fence_before();
-    __syncthreads();       // TMEM, A and the input patch are free for the next tile
-    tc_fence_after();
+    __syncthreads();       // A and the input patch are free for the next tile
     cur = nxt;
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base),
-                 "r"(static_cast<uint32_t>(p.tmem_cols))
-                 : "memory");
   }
 }
 
@@ -269,17 +233,13 @@ int run(const float* in, __half* out, const __half* w, const float* bias, int n,
   const long long total = static_cast<long long>(n) * p.tiles_x * p.tiles_y;
   EDET_CHECK_ARG(total < 0x7fffffffLL, "stem: too many tiles");
   p.total_tiles = static_cast<int>(total);
-  int cols = 32;
-  while (cols < p.npad) cols *= 2;
-  p.tmem_cols = cols;
   p.sched = next_sched_slot();
   if (!p.sched) return EDET_ERR_CUDA;
   const int sms = device_sm_count();
   if (!sms) return EDET_ERR_CUDA;
-  const int smem_bytes = 1024 + kABytes + kBBytes + 2 * kInPad * 4 + 96;
+  const int smem_bytes = 1024 + kABytes + kBBytes + 2 * kInPad * 4 + 32;
   int per_sm = 232448 / (smem_bytes + 1024);
-  if (per_sm > 6) per_sm = 6;
-  if (per_sm * p.tmem_cols > 512) per_sm = 512 / p.tmem_cols;
+  if (per_sm > 4) per_sm = 4;
   const int grid = p.total_tiles < per_sm * sms ? p.total_tiles : per_sm * sms;
   if (act == EDET_ACT_SWISH) return launch<EDET_ACT_SWISH>(p, grid, smem_bytes, stream);
   if (act == EDET_ACT_RELU6) return launch<EDET_ACT_RELU6>(p, grid, smem_bytes, stream);

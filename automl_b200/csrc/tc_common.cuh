@@ -1,4 +1,4 @@
-// Shared pieces of the tcgen05 / TMA kernels (sm_100a): PTX wrappers, UMMA smem descriptors and
+// Shared pieces of the wgmma / TMA kernels (sm_90a): PTX wrappers, wgmma smem descriptors and
 // the host-side tensor-map encoder.
 #pragma once
 #include <cuda.h>
@@ -8,8 +8,7 @@
 namespace edet {
 namespace pwtc {
 
-constexpr int BLOCK_M = 128;
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 
 // pointwise_tc.cu: the GEMM entry point shared by edet_pointwise_conv and edet_class_argmax
 struct ArgmaxArgs {
@@ -85,56 +84,81 @@ __device__ __forceinline__ void tma_store_wait_all() {
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+// ---- warpgroup MMA (wgmma) ------------------------------------------------------------------
+// D[64 x 16] (+)= A[64 x 16] * B[16 x 16]^T, fp16 in, fp32 accumulators in registers, both
+// operands K-major in shared memory (smem descriptors below).  Issued by all 128 threads of a
+// warpgroup.  Fragment of thread t (warp w = (t >> 5) & 3, lane l):
+//   d[0], d[1] = row 16w + l/4,     columns 2(l%4), 2(l%4)+1
+//   d[2], d[3] = row 16w + l/4 + 8, same columns
+//   d[4..7]    = the same two rows, columns + 8
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                           uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wg_mma_m64n16(float* d, uint64_t desc_a, uint64_t desc_b,
+                                              uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+        "+f"(d[7])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
+// Makes the accumulators opaque to the compiler: after wg_wait, so that no read of them is
+// scheduled before the MMAs that write them have completed.
+template <int NT>
+__device__ __forceinline__ void wg_fence_acc(float (&acc)[NT][8]) {
+#pragma unroll
+  for (int j = 0; j < NT; ++j)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) asm volatile("" : "+f"(acc[j][e])::"memory");
 }
-__device__ __forceinline__ void tc_wait_ld() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// One K-major k-block: acc[j] (+)= A[64 rows][16 * ksteps] * B[16j .. 16j+15][...]^T for j < nt.
+// desc_a / desc_b address row 0 of the 64-row A block / the B tile; b_chunk = descriptor units
+// (16 bytes) between 16-row B chunks = the smem row pitch in bytes.  Not waited for.
+template <int NT>
+__device__ __forceinline__ void wg_mma_kblock(float (&acc)[NT][8], uint64_t desc_a,
+                                              uint64_t desc_b, int b_chunk, int nt, int ksteps,
+                                              bool first) {
+  for (int ks = 0; ks < ksteps; ++ks) {
+#pragma unroll
+    for (int j = 0; j < NT; ++j) {
+      // advance 16 halves = 32 bytes inside the swizzle atom: +2 in the >>4 address field
+      if (j < nt)
+        wg_mma_m64n16(acc[j], desc_a + static_cast<uint64_t>(ks * 2),
+                      desc_b + static_cast<uint64_t>(j * b_chunk + ks * 2),
+                      (first && ks == 0) ? 0u : 1u);
+    }
+  }
+}
+// Named barrier over the `threads` threads of barrier `id` (1..15; 0 is __syncthreads).
+__device__ __forceinline__ void named_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// K-major, 128B-swizzled smem matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-// start>>4 [0,14) | LBO>>4 [16,30) = 1 | SBO>>4 [32,46) = 1024>>4 | version [46,48) = 1 |
-// layout [61,64) = 2 (SWIZZLE_128B).
-// The 64B / 32B swizzle variants (layout 4 / 6, SBO 512 / 256) are used for the thin-K layers
-// (K <= 32 / K <= 16) so that a pipeline stage only holds the bytes that exist.
+// K-major swizzled smem matrix descriptor (wgmma layout): start>>4 [0,14) | LBO>>4 [16,30) = 1 |
+// SBO>>4 [32,46) = 8 rows * row pitch | layout [62,64): 1 = SWIZZLE_128B, 2 = 64B, 3 = 32B.
+// The 64B / 32B variants (row pitch 64 / 32 bytes) are used for the thin-K layers (K <= 32 / 16)
+// so that a pipeline stage only holds the bytes that exist.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, int sbo, int layout) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(sbo >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout) << 61;
+  d |= static_cast<uint64_t>(layout) << 62;
   return d;
 }
+// wgmma layout code of a K-major tile whose rows are `block_k` halves
+inline int desc_layout_for(int block_k) { return block_k == 64 ? 1 : (block_k == 32 ? 2 : 3); }
 
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar,

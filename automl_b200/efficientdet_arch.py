@@ -1,4 +1,4 @@
-"""`efficientdet(features, model_name=None, config=None, **kwargs)` on the B200 path.
+"""`efficientdet(features, model_name=None, config=None, **kwargs)` on the H100 path.
 
 Same call surface as /root/reference/efficientdet/efficientdet_arch.py:547-577:
   * raises ValueError when neither model_name nor config is given;

@@ -1,1 +1,1 @@
-"""EfficientNet V1/V2 classifier backbones on the B200 path (reference: efficientnetv2/)."""
+"""EfficientNet V1/V2 classifier backbones on the H100 path (reference: efficientnetv2/)."""

@@ -1,4 +1,4 @@
-"""EfficientNet V1 / V2 backbone on the B200 path: the forward pass of the reference's
+"""EfficientNet V1 / V2 backbone on the H100 path: the forward pass of the reference's
 efficientnetv2/effnetv2_model.py (`EffNetV2Model.call` :595-658) lowered to the C-ABI kernels.
 
   model = effnetv2_model.get_model('efficientnetv2-s', weights=None, batch_size=128, image_size=384)

@@ -1,4 +1,4 @@
-"""Lowers a resolved EfficientDet architecture to a static list of kernel launches on one B200.
+"""Lowers a resolved EfficientDet architecture to a static list of kernel launches on one H100.
 
   * folds inference BatchNorm into the conv weights (reference utils.py:244-326, eps 1e-3),
     casts weights to fp16 / biases to fp32 and uploads them once;
@@ -185,7 +185,7 @@ class Engine(object):
       x_in = cur
       mid = x_in
       # fuse_mbconv_front: blocks whose expanded map is large and whose depthwise is 3x3 stride 2
-      # run the fused front half (expand in TMEM, depthwise from shared memory; the expanded map
+      # run the fused front half (expand in registers, depthwise from shared memory; the expanded map
       # never reaches HBM).  Off by default since round 2: with the three-team pointwise kernel
       # and the TMA-tiled depthwise the separate pair is 1 % faster on the D0 step (4.165 vs
       # 4.204 ms) although it moves 4x the bytes -- the fused kernel serialises TMA -> MMA ->

@@ -44,5 +44,5 @@ def get_fpn_config(fpn_name, min_level, max_level, weight_method):
   if fpn_name in ('bifpn', 'bifpn_dyn'):
     return bifpn_config(min_level, max_level, weight_method)
   if fpn_name == 'qufpn':
-    raise NotImplementedError('qufpn is out of scope for the B200 path')
+    raise NotImplementedError('qufpn is out of scope for the H100 path')
   raise KeyError(fpn_name)

@@ -1,6 +1,6 @@
 """Model registry + attribute-dict config for the EfficientDet forward path.
 
-Host-side mirror of the reference registry so callers of the B200 path can keep
+Host-side mirror of the reference registry so callers of the H100 path can keep
 using `get_efficientdet_config('efficientdet-d0')`, `Config.override('a=1,b.c=2')`
 and friends unchanged.
 

@@ -1,4 +1,4 @@
-"""`ServingDriver` on the B200 path: same call surface as the reference's
+"""`ServingDriver` on the H100 path: same call surface as the reference's
 /root/reference/efficientdet/inference.py:340-554.
 
   driver = inference.ServingDriver('efficientdet-d0', ckpt_path, batch_size=len(imgs))

@@ -91,7 +91,7 @@ def depthwise_conv(x, out, w, bias, act, k, stride, se_sum=None):
 
 
 def conv2d(x, wt, bias, out, act, ksize, stride, residual=None):
-  """k x k 'SAME' convolution on tcgen05: x fp16 [N,H,W,cin], wt fp16 [k*k, cout, cin], bias fp32
+  """k x k 'SAME' convolution on the tensor cores (wgmma): x fp16 [N,H,W,cin], wt fp16 [k*k, cout, cin], bias fp32
   [cout], out fp16 [N,ceil(H/s),ceil(W/s),cout], residual like out or None."""
   n, h, w, cin = x.shape
   cout = wt.shape[1]

@@ -1,4 +1,4 @@
-"""Post-processing call surface of the reference's tf2/postprocess.py on the B200 path.
+"""Post-processing call surface of the reference's tf2/postprocess.py on the H100 path.
 
   generate_detections(params, engine, image_scales, image_ids, flip=False)
       /root/reference/efficientdet/tf2/postprocess.py:530-575, the `nms_configs.pyfunc` branch:

@@ -1,4 +1,4 @@
-"""Size helpers and activation names shared by the host side of the B200 path.
+"""Size helpers and activation names shared by the host side of the H100 path.
 
 Mirrors (reference file:line under /root/reference/efficientdet):
   * utils.py:484-506   parse_image_size  (int | 'WxH' string | (H, W) tuple)

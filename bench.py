@@ -1,6 +1,7 @@
-"""Images/sec of the B200 EfficientDet path on N GPUs of one box (BASELINE.json metric).
+"""Images/sec of the H100 EfficientDet path on N GPUs of one box (BASELINE.json metric).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config d0|d4|d7x|v2s]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 --config picks the BASELINE.json configuration (default d0 = configs[1], the one the metric is
@@ -14,8 +15,13 @@ A "step" = one pass of the hot path (stem .. heads .. pre-NMS .. NMS) over one b
 images per GPU.  `value` is whole-job images/s with inputs already resident in HBM; `e2e` is the
 same metric through the public serving call with HOST buffers (pinned uint8 images copied H2D and
 the [B,100,7] detections copied D2H inside the timed region, three requests in flight).  Inputs
-and the activations written between kernels (GBs per step) exceed the 126 MB L2, so every timed
+and the activations written between kernels (GBs per step) exceed the 50 MB L2, so every timed
 iteration starts with a flushed L2.
+
+--dump-outputs DIR writes, after the timed steps, what the timed path computed in its last step as
+DIR/<name>.npy (float32): the detections [B,100,7] of a detector, or a fixed seeded sample of 2^20
+elements of the EfficientNetV2 head feature map.  Inputs and weights are seeded, so two builds run
+with the same arguments can be compared output for output.
 
 --impl reference times the reference's CPU implementation of the path.  TensorFlow is probed at
 run time (it is not installable offline); without it the arm runs the oracle port
@@ -73,7 +79,7 @@ def workload_config(cfg, world):
     what = '%s %dx%d batch %d/GPU: stem, %s' % (cfg['model'], s, s, cfg['batch'], cfg['blocks'])
   return {'workload': what, 'global_batch': world * cfg['batch'],
           'parallelism': 'batch-shard x%d' % world,
-          'l2': 'inputs and per-step activations (GBs) exceed the 126 MB L2, so every timed '
+          'l2': 'inputs and per-step activations (GBs) exceed the 50 MB L2, so every timed '
                 'iteration starts with a flushed L2'}
 
 
@@ -129,7 +135,7 @@ def measured_peaks():
     with open(path) as f:
       d = json.load(f)
     return d['hbm_gbs'], d.get('bf16_tflops_sustained', d.get('bf16_tflops')), 'measured'
-  return 6650.0, 1400.0, 'fallback'
+  return 3350.0, 989.0, 'H100 SXM data sheet (HBM3, dense fp16)'
 
 
 # ---- the reference's CPU implementation -----------------------------------------------------------
@@ -279,24 +285,6 @@ def roofline_from_rows(rows, exclude=('nms_v5',)):
   return roof, kinds, total_ms
 
 
-def attach_traffic(roof, cfg_name):
-  """DRAM bytes of the dominant family per forward from the committed ncu capture of this same
-  command (profiles/r2_traffic_<config>.json, written by scripts/make_profiles.py)."""
-  for rnd in ('r2', 'r1'):
-    path = os.path.join(ROOT, 'profiles', '%s_traffic_%s.json' % (rnd, cfg_name))
-    if not os.path.exists(path) and cfg_name == 'd0':
-      path = os.path.join(ROOT, 'profiles', '%s_traffic.json' % rnd)
-    if not os.path.exists(path):
-      continue
-    with open(path) as f:
-      t = json.load(f).get('per_forward', {}).get(roof['kernel'])
-    if t:
-      roof['traffic'] = int((t['dram_read_MB'] + t['dram_write_MB']) * 1e6)
-      roof['traffic_source'] = ('%s (ncu dram__bytes_read.sum + dram__bytes_write.sum, family sum '
-                                'per forward)' % os.path.relpath(path, ROOT))
-      return
-
-
 # ---- our arm ---------------------------------------------------------------------------------------
 def main():
   ap = argparse.ArgumentParser()
@@ -307,6 +295,7 @@ def main():
   ap.add_argument('--config', default='d0', choices=sorted(CONFIGS))
   ap.add_argument('--no-cpu-baseline', action='store_true')
   ap.add_argument('--profile-out', default='')
+  ap.add_argument('--dump-outputs', default='', metavar='DIR')
   args = ap.parse_args()
   cfg = CONFIGS[args.config]
 
@@ -369,6 +358,9 @@ def main():
     api = ('inference.ServingDriver.submit(uint8 [%d,%d,%d,3] pinned host).result() -> numpy '
            'detections, three requests in flight (H2D, device pre-process, network, NMS, all-gather, '
            'D2H per step)' % ((batch,) + cfg['raw_hw']))
+    def outputs():
+      eng.wait_detections()
+      return {'detections': eng.detections.float()}
     profile = lambda: eng.profile_ops(iters=3)
     launches = eng.launches_per_forward
     extra = lambda: {'nms_full_queue_images': eng.nms_fallback_count()}
@@ -407,6 +399,12 @@ def main():
     launches = len(model._ops)  # pylint: disable=protected-access
     extra = lambda: {}
 
+    def outputs():
+      head = model.endpoints['head_1x1'].reshape(-1)
+      idx = np.sort(np.random.default_rng(0).choice(head.numel(), size=1 << 20, replace=False))
+      return {'head_1x1_sample': head[torch.from_numpy(idx).to(head.device)].float(),
+              'head_1x1_sample_index': torch.from_numpy(idx.astype(np.float64))}
+
   def timed(loop, steps, warm):
     loop(warm)
     if world > 1:
@@ -437,6 +435,11 @@ def main():
   ms_e2e = timed(e2e_loop, args.steps, 3)
   clocks = sampler.stop() if rank == 0 else None
 
+  if args.dump_outputs and rank == 0:
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    for name, t in outputs().items():
+      np.save(os.path.join(args.dump_outputs, name + '.npy'), t.cpu().numpy())
+
   value = world * batch * args.steps / (ms_dev / 1000.0)
   e2e_value = world * batch * args.steps / (ms_e2e / 1000.0)
 
@@ -444,7 +447,6 @@ def main():
   if rank == 0:
     rows = profile()
     roofline, kinds, total_ms = roofline_from_rows(rows)
-    attach_traffic(roofline, args.config)
     if args.profile_out:
       with open(args.profile_out, 'w') as f:
         json.dump({'ops': rows, 'kinds': roofline['per_kind'], 'sum_ms': total_ms}, f, indent=1)

@@ -1,5 +1,5 @@
 /*
- * automl_b200 C ABI: the sm_100a kernels behind the EfficientDet forward path.
+ * automl_b200 C ABI: the sm_90a kernels behind the EfficientDet forward path.
  *
  * The reference (google/automl, /root/reference/efficientdet) has no plugin / FFI layer: its
  * hot path bottoms out in TensorFlow ops.  Each entry point below replaces the TF op(s) a
@@ -50,7 +50,7 @@ enum {
 
 /* Pointwise implementation selector. */
 enum {
-  EDET_PW_TCGEN05 = 0, /* TMA -> smem -> tcgen05.mma -> TMEM -> epilogue -> TMA store */
+  EDET_PW_TCGEN05 = 0, /* TMA -> smem -> wgmma -> registers -> epilogue -> TMA store */
   EDET_PW_SIMT = 1     /* plain CUDA-core kernel, kept only as an on-device cross-check */
 };
 
@@ -59,12 +59,11 @@ const char* edet_last_error(void);
 /* Process-wide implementation switches, for A/B measurements and tests only (results are the same
  * for every setting).  Options: "dw_impl" = 0 (default: TMA-tiled depthwise kernel where eligible,
  * register-tiled kernel otherwise) | 1 (register-tiled kernel only); "pw_teams" = 0 (default:
- * three epilogue teams) | 2 | 3; "stem_impl" = 0 (default: tensor-core stem) | 1 (CUDA-core stem);
+ * two consumer warpgroups) | 2 | 3; "stem_impl" = 0 (default: tensor-core stem) | 1 (CUDA-core stem);
  * "sepconv_impl" = 0 (default: TMA-staged input tile for c <= 64, one buffer, four CTAs per SM) |
  * 1 (loads from global) | 2 (TMA, two buffers, three CTAs per SM);
- * "pw_smem_kb" = 0 (default: 99 KiB per pointwise CTA where that keeps the TMA ring >= 4 deep, so
- * that one CTA shares an SM with an NMS CTA of the previous batch; else 113) | 64..113;
- * "persist_slack" = CTAs a persistent kernel leaves out of its two-per-SM grid (default 0). */
+ * "pw_smem_kb" = 0 (default: 227 KiB, one pointwise CTA per SM) | 64..227;
+ * "persist_slack" = CTAs a persistent kernel leaves out of its grid (default 0). */
 int edet_set_option(const char* name, int value);
 int edet_get_option(const char* name, int* value);
 /* Number of SMs / compute capability of the current device (major*10+minor). */
@@ -93,7 +92,7 @@ int edet_stem_conv(const float* in, edet_half* out, const edet_half* w, const fl
                    int n, int h, int wd, int cout, int act, edet_stream_t stream);
 
 /* k x k convolution 'SAME' (ksize in {1,3,5}, stride in {1,2}) + bias (BN folded) + act
- * (+ residual) as an implicit GEMM on tcgen05: the Fused-MBConv convolutions of EfficientNetV2.
+ * (+ residual) as an implicit GEMM on the tensor cores (wgmma): the Fused-MBConv convolutions of EfficientNetV2.
  * Replaces Conv2D k x k + BN (+ act) (+ skip)  efficientnetv2/effnetv2_model.py:331-341, 355-364,
  * 387-404 (FusedMBConvBlock), residual :270-277.
  *   in  half [n, h, w, cin]                 wt  half [ksize*ksize][cout][cin] (tap-major, cin
@@ -105,8 +104,8 @@ int edet_conv2d(const edet_half* in, const edet_half* wt, const float* bias,
                 int ksize, int stride, int act, edet_stream_t stream);
 
 /* Fused front half of an MBConv block: expand 1x1 + BN + act  ->  depthwise kxk 'SAME' + BN +
- * act (+ SE squeeze), the expanded [N,H,W,cmid] tensor never leaves the SM (tcgen05 accumulators
- * in TMEM -> fp16 tile in shared memory -> depthwise).  Same results as edet_pointwise_conv
+ * act (+ SE squeeze), the expanded [N,H,W,cmid] tensor never leaves the SM (wgmma accumulators
+ * in registers -> fp16 tile in shared memory -> depthwise).  Same results as edet_pointwise_conv
  * followed by edet_depthwise_conv (the expanded value is rounded to fp16 in both).
  * Replaces: backbone/efficientnet_model.py:303-333 (the two convs + BNs), :387-391 (their use in
  * MBConvBlock._call) and the reduce_mean of :192.
@@ -191,7 +190,7 @@ typedef struct {
 int edet_fuse_dw(const edet_fuse_input* h_inputs, int n_inputs, const float* dw_w,
                  edet_half* out, int n, int h, int wd, int c, int act, edet_stream_t stream);
 
-/* Fused separable convolution of a head tower layer (tcgen05):
+/* Fused separable convolution of a head tower layer (wgmma):
  *   out = post_act( pointwise( depthwise3x3( input ) ) + bias )
  * i.e. a depthwise conv followed by edet_pointwise_conv without the [n,h,w,c] intermediate in HBM
  * (the depthwise result is rounded to fp16 in shared memory, exactly as the pair rounds it in

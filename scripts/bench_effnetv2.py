@@ -1,4 +1,4 @@
-"""BASELINE config 3: EfficientNetV2-S 384x384 backbone-only, batch 128, one B200 (not the bench.py
+"""BASELINE config 3: EfficientNetV2-S 384x384 backbone-only, batch 128, one H100 (not the bench.py
 headline; a reported parity-case number).  CUDA graph replay, CUDA events, 20 steps after 5."""
 import json
 import os

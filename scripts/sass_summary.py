@@ -1,7 +1,7 @@
-"""Per-kernel SASS evidence for the Blackwell-native paths: counts of the tcgen05 / TMEM / TMA
-instructions (UTC*MMA, LDTM / STTM, UTMALDG / UTMASTG / UBLKCP), legacy tensor instructions (HMMA)
-and the packed-fp32 / MUFU instructions in every kernel of libautoml_b200.so.
-usage: python scripts/sass_summary.py > profiles/r2_sass_summary.md   (no GPU needed)"""
+"""Per-kernel SASS evidence for the Hopper-native paths: counts of the wgmma (HGMMA), TMA
+(UTMALDG / UTMASTG / UBLKCP) and mbarrier (SYNCS) instructions, legacy tensor instructions (HMMA)
+and the MUFU / memory instructions in every kernel of libautoml_b200.so.
+usage: python scripts/sass_summary.py > sass_summary.md   (no GPU needed)"""
 import collections
 import os
 import re
@@ -10,7 +10,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, 'automl_b200', 'csrc', 'libautoml_b200.so')
-COLS = ['UTC*MMA', 'LDTM', 'UTMALDG', 'UTMASTG', 'SYNCS', 'HMMA', 'FFMA2', 'MUFU', 'LDG', 'LDS', 'total']
+COLS = ['HGMMA', 'UTMALDG', 'UTMASTG', 'SYNCS', 'HMMA', 'MUFU', 'LDG', 'LDS', 'total']
 
 
 def main():
@@ -26,15 +26,13 @@ def main():
     if cur is not None and m:
       op = m.group(1).split('.')[0]
       cur['total'] += 1
-      if re.match(r'UTC\w*MMA', op):
-        cur['UTC*MMA'] += 1
-      elif op in ('LDTM', 'STTM', 'UTMALDG', 'UTMASTG', 'UBLKCP', 'SYNCS', 'HMMA', 'FFMA2', 'MUFU', 'LDG', 'LDS'):
+      if op in ('HGMMA', 'UTMALDG', 'UTMASTG', 'UBLKCP', 'SYNCS', 'HMMA', 'MUFU', 'LDG', 'LDS'):
         cur[op] += 1
   names = subprocess.run(['c++filt'], input='\n'.join(kernels), stdout=subprocess.PIPE, text=True).stdout.splitlines()
   arch = re.findall(r'arch = (sm_\w+)', sass)
   print('# SASS instruction counts per kernel (`cuobjdump -sass libautoml_b200.so`, %s only)\n' % ', '.join(sorted(set(arch))))
-  print('`UTC*MMA` = tcgen05.mma, `LDTM` = tcgen05.ld, `UTMALDG` / `UTMASTG` = TMA tensor load / store, '
-        '`SYNCS` = mbarrier ops, `HMMA` = legacy mma.sync (none expected), `FFMA2` = packed fp32 FMA.\n')
+  print('`HGMMA` = wgmma.mma_async, `UTMALDG` / `UTMASTG` = TMA tensor load / store, '
+        '`SYNCS` = mbarrier ops, `HMMA` = legacy mma.sync (none expected).\n')
   print('| kernel | ' + ' | '.join(COLS) + ' |')
   print('|---|' + '---:|' * len(COLS))
   fam = collections.OrderedDict()

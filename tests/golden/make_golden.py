@@ -82,6 +82,20 @@ def main():
   cases['methods'] = np.asarray([json.dumps(m) for m in methods])
   np.savez_compressed(os.path.join(OUT, 'nms_np_nms.npz'), **cases)
 
+  # nms_np.nms on seeded random candidate sets, every method with its defaults
+  rnd = {}
+  rng7 = np.random.default_rng(7)
+  for k in (3, 64, 400):
+    c = rng7.uniform(0, 300, size=(k, 2))
+    wh = rng7.uniform(5, 120, size=(k, 2))
+    dets = np.column_stack([c - wh / 2, c + wh / 2,
+                            rng7.permutation(np.linspace(0.01, 0.99, k))]).astype(np.float32)
+    rnd['dets_%d' % k] = dets
+    for method in ('hard', 'diou', 'gaussian', 'linear'):
+      cfg = dict(method=method, iou_thresh=None, score_thresh=0.0, sigma=None)
+      rnd['out_%d_%s' % (k, method)] = np.asarray(nms_np.nms(dets.copy(), dict(cfg)), np.float32)
+  np.savez_compressed(os.path.join(OUT, 'nms_np_nms_random.npz'), **rnd)
+
   # per_class_nms goldens
   pc = {}
   for ci, k in enumerate([50, 600, 5000]):

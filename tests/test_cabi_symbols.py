@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads without a GPU, and exports every symbol that
+"""The C-ABI library builds for sm_90a, loads without a GPU, and exports every symbol that
 include/automl_b200.h declares (and ctypes signatures exist for all of them)."""
 import ctypes
 import os

@@ -97,8 +97,8 @@ def test_pointwise_conv(case, impl_name):
     (1, 300, 64, 88, utils.ACT_SWISH, True, False),        # 88 = 2 units + a 24-column tail (16 + 8)
 ])
 def test_pointwise_epilogue_teams_agree(case):
-  """The two epilogue organisations of pointwise_tc_kernel (two teams x 64-column chunks, three
-  teams x 32-column units) read the same accumulators and do the same fp32 epilogue arithmetic:
+  """The two organisations of pointwise_tc_kernel (two or three consumer warpgroups taking tiles in
+  turn, each with its own stage ring) do the same MMAs and the same fp32 epilogue arithmetic:
   bit-identical outputs."""
   ops = _ops()
   batch, rows, k, nout, act, has_res, per_image = case
@@ -300,8 +300,8 @@ def test_se_fc(shape):
 @pytest.mark.parametrize('hw,cout,n', [((64, 64), 32, 2), ((33, 47), 48, 2), ((8, 8), 64, 1),
                                       ((127, 129), 40, 1), ((200, 96), 56, 3), ((5, 3), 24, 1)])
 def test_stem_conv(hw, cout, n, impl):
-  """Both stem kernels (implicit GEMM on tcgen05 with the float32 input split into fp16 hi + lo;
-  CUDA-core FFMA2) against the float64 oracle: even / odd sizes (asymmetric 'SAME' padding),
+  """Both stem kernels (implicit GEMM on the tensor cores (wgmma) with the float32 input split into fp16 hi + lo;
+  CUDA-core FFMA) against the float64 oracle: even / odd sizes (asymmetric 'SAME' padding),
   widths that are not multiples of 16 (N padding), several tiles per CTA."""
   ops = _ops()
   h, w = hw
