@@ -4,14 +4,16 @@
 //
 // Structure (persistent CTAs, one per SM, warp-specialised):
 //   warpgroup 0        : warp 0 / lane 0 is the TMA producer -- cp.async.bulk.tensor (3-D maps,
-//                        128B / 64B / 32B swizzle) of the A tile [64 x block_k] and the W tile
+//                        128B / 64B / 32B swizzle) of the A tile [64 x block_k] and, unless all
+//                        of W is resident in smem (kResidentWBytes), the W tile
 //                        [block_n x block_k] into the smem stage ring of the consumer that owns
 //                        the tile (mbarrier complete_tx).  Each consumer has a ring of its own, so
 //                        it sees every phase of its stage barriers (a consumer that skipped the
 //                        other's stages could meet a barrier two phases behind, whose parity looks
 //                        complete).  Out-of-bounds rows / K tail are zero-filled by TMA.
 //   warpgroups 1..TEAMS: consumers.  Tile i of the CTA belongs to consumer i % TEAMS, which runs
-//                        the wgmma main loop (m64 x n16 x k16, fp32 accumulators in registers) and
+//                        the wgmma main loop (one m64 x block_n x k16 per k-step, fp32
+//                        accumulators in registers, one k-block of MMAs in flight) and
 //                        then its own epilogue: +bias -> activation -> (+residual) -> fp16 ->
 //                        128B-swizzled staging slab -> TMA store (clips the ragged M / N edges).
 //                        While one consumer is in its MUFU-bound epilogue the other one's MMAs run.
@@ -21,6 +23,8 @@
 //   2*(batch*rows*k + batch*rows*nout [+ same for residual]) + 2*wbatch*nout*k   (SURVEY 8d).
 #include <math_constants.h>
 
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace edet {
@@ -28,17 +32,20 @@ namespace pwtc {
 
 constexpr int BLOCK_M = 64;         // rows per tile = the M of one wgmma
 constexpr int kMaxBlockN = 128;     // accumulator columns per consumer thread: kMaxBlockN / 2
-constexpr int kNT = kMaxBlockN / 16;
 template <int TEAMS>
 struct Epi {
   static constexpr int kThreads = 128 * (1 + TEAMS);
 };
 constexpr int kStoreCols = 64;
 constexpr int kSlabBytes = BLOCK_M * kStoreCols * 2;   // [64 rows][64 cols] fp16, 128B swizzle
-constexpr int kSlabsPerTeam = kMaxBlockN / kStoreCols;
 constexpr int kMaxStages = 9;   // 4 + 4 (two consumers) or 3 + 3 + 3
 constexpr int kRing = 4;          // tile-index ring entries (power of two)
 constexpr int kSmemLimit = 227 * 1024;                   // one CTA per SM
+// Weights of at most this many (padded, swizzled) bytes stay in shared memory for the life of the
+// CTA: every D0 layer up to blocks_8, the BiFPN layers and both predict layers (the class head,
+// 9 anchors x 96 x 64 halves, is exactly this size).  What is left still holds the staging slabs
+// and at least two A stages per consumer.
+constexpr int kResidentWBytes = 108 * 1024;
 
 struct Params {
   int batch, rows, k, nout, nout_pad8;
@@ -46,6 +53,10 @@ struct Params {
   int team_stages;    // stages of each consumer's own ring: num_stages / TEAMS
   int block_k;        // 64 / 32 / 16 halves per k-block == 128B / 64B / 32B swizzled smem rows
   int a_stage_bytes, b_stage_bytes;
+  int stage_bytes;    // ring bytes per stage: A, plus the W tile unless W is resident
+  int w_resident;     // 1: all of W (wbatch == 1) lives in smem, loaded once per CTA
+  int slab_sets;      // staging-slab sets per consumer (2: a tile's stores overlap the next epilogue)
+  int slab_set_bytes; // one set: ceil(block_n / 64) slabs of [64 rows][64 cols]
   int desc_sbo;       // byte distance between 8-row groups in smem (8 * row pitch)
   int desc_layout;    // wgmma layout type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
   int wbatch, ldr;
@@ -111,9 +122,12 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
   // 1024-byte alignment for the swizzle atoms.
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
-  uint8_t* smem_store = smem + p.num_stages * stage_bytes;   // [TEAMS][kSlabsPerTeam] slabs
-  float* smem_bias = reinterpret_cast<float*>(smem_store + TEAMS * kSlabsPerTeam * kSlabBytes);
+  const int stage_bytes = p.stage_bytes;
+  // resident W: [num_n_blocks][num_k_blocks] boxes of b_stage_bytes (empty unless w_resident)
+  uint8_t* smem_w = smem + p.num_stages * stage_bytes;
+  const int w_bytes = p.w_resident ? p.num_n_blocks * p.num_k_blocks * p.b_stage_bytes : 0;
+  uint8_t* smem_store = smem_w + w_bytes;   // [TEAMS][slab_sets] slab sets
+  float* smem_bias = reinterpret_cast<float*>(smem_store + TEAMS * p.slab_sets * p.slab_set_bytes);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_bias + p.bias_floats);
   uint64_t* full_bar = bars;                       // [kMaxStages]
   uint64_t* empty_bar = bars + kMaxStages;         // [kMaxStages]
@@ -125,9 +139,11 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
   uint64_t* ring_empty = ring_full + kRing;        // [kRing] consumers -> producer
   // [kRing] x {tile, batch entry, M block, N block}: the producer decodes each tile once (its two
   // integer divisions) and the consumers read the coordinates with one 16-byte load
-  volatile int4* tile_ring = reinterpret_cast<volatile int4*>(ring_empty + kRing);
+  uint64_t* w_full = ring_empty + kRing;          // [2]: [0] resident W landed, [1] padding
+  volatile int4* tile_ring = reinterpret_cast<volatile int4*>(w_full + 2);
 
-  const int warp = threadIdx.x >> 5;
+  // warp-uniform as far as ptxas can tell (see the tile-ring broadcast below)
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
@@ -139,6 +155,7 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
       mbar_init(smem_u32(&ring_full[s]), 1);
       mbar_init(smem_u32(&ring_empty[s]), TEAMS);  // one arrive per consumer warpgroup
     }
+    mbar_init(smem_u32(&w_full[0]), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
@@ -148,14 +165,26 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
   for (int i = threadIdx.x; i < p.bias_floats; i += blockDim.x)
     smem_bias[i] = i < p.nout ? __ldg(p.bias + i) : 0.f;
   __syncthreads();
+  // after the wait: with batch 1 the SE-scaled weights are a single [nout][K] matrix (wbatch 1)
+  // that the previous kernel writes
   pdl_wait_prior();          // everything above overlapped the previous kernel's tail
 
   if (warp == 0) {
     // ===================== TMA producer =====================
     if (lane == 0) {
+      const uint32_t w_box_bytes = static_cast<uint32_t>(p.block_n * p.block_k * 2);
+      if (p.w_resident) {
+        const uint32_t wb = smem_u32(&w_full[0]);
+        mbar_expect_tx(wb, w_box_bytes * p.num_n_blocks * p.num_k_blocks);
+        for (int nb = 0; nb < p.num_n_blocks; ++nb)
+          for (int kb = 0; kb < p.num_k_blocks; ++kb)
+            tma_load_3d(smem_u32(smem_w + (nb * p.num_k_blocks + kb) * p.b_stage_bytes), &map_w,
+                        wb, kb * p.block_k, nb * p.block_n, 0);
+      }
       int stage_of[TEAMS] = {}, phase_of[TEAMS] = {};   // per consumer ring
-      // bytes the two TMA boxes deliver (the B slot may be padded to 1 KiB)
-      const uint32_t tx_bytes = static_cast<uint32_t>(p.a_stage_bytes + p.block_n * p.block_k * 2);
+      // bytes the TMA boxes of one stage deliver (the B slot may be padded to 1 KiB)
+      const uint32_t tx_bytes =
+          static_cast<uint32_t>(p.a_stage_bytes) + (p.w_resident ? 0u : w_box_bytes);
       bool exhausted = false;
       for (int i = 0;; ++i) {
         int t = p.total_tiles;
@@ -184,8 +213,9 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
           mbar_expect_tx(fb, tx_bytes);
           uint8_t* sa = smem + s * stage_bytes;
           tma_load_3d(smem_u32(sa), &map_a, fb, kb * p.block_k, tc.m_blk * BLOCK_M, tc.b);
-          tma_load_3d(smem_u32(sa + p.a_stage_bytes), &map_w, fb, kb * p.block_k,
-                      tc.n_blk * p.block_n, wb);
+          if (!p.w_resident)
+            tma_load_3d(smem_u32(sa + p.a_stage_bytes), &map_w, fb, kb * p.block_k,
+                        tc.n_blk * p.block_n, wb);
           if (++stage == p.team_stages) {
             stage = 0;
             phase ^= 1;
@@ -201,8 +231,14 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
     const int wtid = threadIdx.x & 127;
     const int r0 = 16 * (warp & 3) + (lane >> 2);   // rows r0 and r0 + 8 of the tile
     const int cq = 2 * (lane & 3);                  // column pair inside each 8-column group
-    uint8_t* my_slabs = smem_store + team * kSlabsPerTeam * kSlabBytes;
-    const int b_chunk = p.block_k * 2;              // descriptor units between 16-row B chunks
+    uint8_t* team_slabs = smem_store + team * p.slab_sets * p.slab_set_bytes;
+    if (p.w_resident) mbar_wait(smem_u32(&w_full[0]), 0);
+    // The tile loop for NT 16-column groups: one wgmma of N = 16 NT per k-step over the whole N
+    // tile.  W rows of a ragged last tile past nout are TMA zero fill; their columns are computed
+    // but not stored.
+    auto consume = [&](auto nt_const) {
+    constexpr int NT = decltype(nt_const)::value;
+    int my_tiles = 0;         // tiles this consumer has run: selects the staging-slab set
     int stage = 0;            // in this consumer's ring: stages team * team_stages ..
     uint32_t phase = 0;
     auto advance = [&]() {
@@ -214,7 +250,13 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
     for (int iter = 0;; ++iter) {
       const int slot = iter & (kRing - 1);
       mbar_wait(smem_u32(&ring_full[slot]), static_cast<uint32_t>(iter / kRing) & 1u);
-      const int4 e = const_cast<const int4*>(tile_ring)[slot];
+      int4 e = const_cast<const int4*>(tile_ring)[slot];
+      // Broadcast from lane 0: a value ptxas cannot prove warp-uniform puts the tile loop, and
+      // with it every wgmma, on a divergent path, and ptxas then serialises the wgmmas (C7520).
+      e.x = __shfl_sync(0xffffffffu, e.x, 0);
+      e.y = __shfl_sync(0xffffffffu, e.y, 0);
+      e.z = __shfl_sync(0xffffffffu, e.z, 0);
+      e.w = __shfl_sync(0xffffffffu, e.w, 0);
       named_sync(1 + team, 128);
       if (wtid == 0) mbar_arrive(smem_u32(&ring_empty[slot]));
       const int t = e.x;
@@ -225,32 +267,44 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
       tc.m_blk = e.z;
       tc.n_blk = e.w;
       const int n0 = tc.n_blk * p.block_n;
-      // only the columns that exist in the output are worth MMAs and an epilogue (rounded up to
-      // the 16-column MMA granule); the rest of a ragged last N tile is skipped
+      // only the columns that exist in the output are worth an epilogue (rounded up to 16); the
+      // rest of a ragged last N tile is skipped
       const int n_valid = min(p.block_n, ((p.nout - n0 + 15) >> 4) << 4);
       const int nt = n_valid >> 4;
-      float acc[kNT][8];
+      float acc[NT][8];
 #pragma unroll
-      for (int j = 0; j < kNT; ++j)
+      for (int j = 0; j < NT; ++j)
 #pragma unroll
         for (int q = 0; q < 8; ++q) acc[j][q] = 0.f;
+      // One k-block of MMAs stays in flight: the stage of k-block kb - 1 is released once the
+      // MMAs of kb are issued and those of kb - 1 have completed.
+      int prev_s = -1;
       for (int kb = 0; kb < p.num_k_blocks; ++kb) {
         const int s = team * p.team_stages + stage;
         mbar_wait(smem_u32(&full_bar[s]), phase);
         uint8_t* sa = smem + s * stage_bytes;
+        uint8_t* sb = p.w_resident
+                          ? smem_w + (tc.n_blk * p.num_k_blocks + kb) * p.b_stage_bytes
+                          : sa + p.a_stage_bytes;
         const uint64_t da = make_smem_desc(smem_u32(sa), p.desc_sbo, p.desc_layout);
-        const uint64_t db = make_smem_desc(smem_u32(sa + p.a_stage_bytes), p.desc_sbo, p.desc_layout);
+        const uint64_t db = make_smem_desc(smem_u32(sb), p.desc_sbo, p.desc_layout);
         const int k_rem = p.k - kb * p.block_k;
         const int ksteps = k_rem >= p.block_k ? p.block_k / MMA_K : (k_rem + MMA_K - 1) / MMA_K;
         wg_fence();
-        wg_mma_kblock<kNT>(acc, da, db, b_chunk, nt, ksteps, kb == 0);
+        wg_mma_kblock_wide<NT>(acc, da, db, ksteps, kb == 0);
         wg_commit();
-        wg_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));   // this warp is done with it
+        wg_wait<1>();
+        if (prev_s >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_s]));   // this warp is done with it
+        }
+        prev_s = s;
         advance();
       }
-      wg_fence_acc<kNT>(acc);
+      wg_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_s]));
+      wg_fence_acc<NT>(acc);
       const int row0 = tc.m_blk * BLOCK_M + r0;
       if constexpr (EPI == EPI_ARGMAX) {
         // Class head fused with the class half of pre-NMS (tf2/postprocess.py:88-156 with
@@ -299,11 +353,19 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
             res_row[r] = p.residual +
                          (static_cast<size_t>(tc.b) * p.rows + (ok[r] ? row0 + 8 * r : 0)) * p.ldr;
         }
-        // the slabs are free once this consumer's previous stores have read them
-        if (wtid == 0) tma_store_wait_read<0>();
+        // a slab set is free once the stores that last read it (this consumer's previous tile, or
+        // the one before that with two sets) have read it
+        uint8_t* my_slabs = team_slabs + (my_tiles % p.slab_sets) * p.slab_set_bytes;
+        ++my_tiles;
+        if (wtid == 0) {
+          if (p.slab_sets == 2)
+            tma_store_wait_read<1>();
+          else
+            tma_store_wait_read<0>();
+        }
         named_sync(1 + team, 128);
 #pragma unroll
-        for (int j = 0; j < kNT; ++j) {
+        for (int j = 0; j < NT; ++j) {
           if (j < nt) {
             const int colt = 16 * j + cq;            // tile column of acc[j][0]
             const float2 b_lo = *reinterpret_cast<const float2*>(smem_bias + n0 + colt);
@@ -339,6 +401,18 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
         }
       }
     }
+    };
+    // block_n is a multiple of 32 (pick_block_n); the width is uniform over the kernel
+    if constexpr (EPI == EPI_ARGMAX) {
+      consume(std::integral_constant<int, kArgmaxCols / 16>{});
+    } else {
+      switch (p.block_n >> 5) {
+        case 1: consume(std::integral_constant<int, 2>{}); break;
+        case 2: consume(std::integral_constant<int, 4>{}); break;
+        case 3: consume(std::integral_constant<int, 6>{}); break;
+        default: consume(std::integral_constant<int, 8>{}); break;
+      }
+    }
     if (wtid == 0) tma_store_wait_all();
   }
 }
@@ -348,7 +422,7 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
 // the next tile), the A tile of the extra tiles comes from L2.  The class-head arg-max epilogue
 // needs one anchor (kArgmaxCols columns) per tile.
 static int pick_block_n(int nout) {
-  if (nout <= kMaxBlockN) return ((nout + 15) / 16) * 16;
+  if (nout <= kMaxBlockN) return ((nout + 31) / 32) * 32;   // a wgmma width (wg_mma_kblock_wide)
   return kMaxBlockN;
 }
 
@@ -405,12 +479,26 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   p.block_k = k <= 16 ? 16 : (k <= 32 ? 32 : 64);
   p.a_stage_bytes = BLOCK_M * p.block_k * 2;
   p.b_stage_bytes = ((p.block_n * p.block_k * 2 + 1023) / 1024) * 1024;
-  const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
-  const int fixed = teams * kSlabsPerTeam * kSlabBytes + p.bias_floats * 4 +
-                    (2 * kMaxStages + 2 * kRing) * 8 + 16 * kRing;
+  p.num_k_blocks = ceil_div(k, p.block_k);
+  // Shared weights small enough stay resident: the ring then carries only A, and the class head
+  // reads each A tile from L2 once per anchor instead of once per anchor AND W tile.  Per-image
+  // (SE-scaled) weights keep streaming with A.
+  const int w_bytes = p.num_n_blocks * p.num_k_blocks * p.b_stage_bytes;
+  p.w_resident = wbatch == 1 && w_bytes <= kResidentWBytes;
+  p.stage_bytes = p.a_stage_bytes + (p.w_resident ? 0 : p.b_stage_bytes);
+  // the arg-max epilogue stores nothing through TMA: no staging slabs
+  p.slab_set_bytes = am ? 0 : ceil_div(p.block_n, kStoreCols) * kSlabBytes;
   const int opt_kb = option_pw_smem_kb();
   const int limit = opt_kb ? opt_kb * 1024 : kSmemLimit;
-  int stages = (limit - 1024 - fixed) / stage_bytes;
+  auto fixed_bytes = [&](int sets) {
+    return (p.w_resident ? w_bytes : 0) + teams * sets * p.slab_set_bytes + p.bias_floats * 4 +
+           (2 * kMaxStages + 2 * kRing + 2) * 8 + 16 * kRing;
+  };
+  // Two slab sets per consumer (the stores of one tile drain while the next epilogue writes) when
+  // that still leaves each consumer three stages; else one.
+  p.slab_sets = (limit - 1024 - fixed_bytes(2)) / p.stage_bytes >= 3 * teams ? 2 : 1;
+  const int fixed = fixed_bytes(p.slab_sets);
+  int stages = (limit - 1024 - fixed) / p.stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   p.team_stages = stages / teams;            // each consumer's own ring
   EDET_CHECK_ARG(p.team_stages >= 2, "pointwise_tc: block_n %d leaves <2 pipeline stages per consumer",
@@ -419,8 +507,7 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   p.num_stages = stages;
   p.desc_layout = desc_layout_for(p.block_k);
   p.desc_sbo = 8 * p.block_k * 2;
-  p.num_k_blocks = ceil_div(k, p.block_k);
-  const int smem_bytes = 1024 + stages * stage_bytes + fixed;
+  const int smem_bytes = 1024 + stages * p.stage_bytes + fixed;
 
   CUtensorMap ma, mw, mo;
   int rc;
