@@ -11,10 +11,11 @@
 //                        it sees every phase of its stage barriers (a consumer that skipped the
 //                        other's stages could meet a barrier two phases behind, whose parity looks
 //                        complete).  Out-of-bounds rows / K tail are zero-filled by TMA.
-//   warpgroups 1..TEAMS: consumers.  Tile i of the CTA belongs to consumer i % TEAMS, which runs
-//                        the wgmma main loop (one m64 x block_n x k16 per k-step, fp32
-//                        accumulators in registers, one k-block of MMAs in flight) and
-//                        then its own epilogue: +bias -> activation -> (+residual) -> fp16 ->
+//   warpgroups 1..TEAMS: consumers.  Work unit i of the CTA (up to 8 consecutive 64-row M blocks
+//                        of one image, see Params) belongs to consumer i % TEAMS, which runs, per
+//                        tile of the unit, the wgmma main loop (one m64 x block_n x k16 per
+//                        k-step, fp32 accumulators in registers, one k-block of MMAs in flight)
+//                        and then its own epilogue: +bias -> activation -> (+residual) -> fp16 ->
 //                        128B-swizzled staging slab -> TMA store (clips the ragged M / N edges).
 //                        While one consumer is in its MUFU-bound epilogue the other one's MMAs run.
 //
@@ -23,6 +24,7 @@
 //   2*(batch*rows*k + batch*rows*nout [+ same for residual]) + 2*wbatch*nout*k   (SURVEY 8d).
 #include <math_constants.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -38,14 +40,24 @@ struct Epi {
 };
 constexpr int kStoreCols = 64;
 constexpr int kSlabBytes = BLOCK_M * kStoreCols * 2;   // [64 rows][64 cols] fp16, 128B swizzle
-constexpr int kMaxStages = 9;   // 4 + 4 (two consumers) or 3 + 3 + 3
-constexpr int kRing = 4;          // tile-index ring entries (power of two)
+// Stages are sized from bytes: each consumer gets enough for kTeamInFlightBytes of loads (16
+// stages of a thin-K 2 KB A tile, 4 of a 128B-swizzled 8 KB one), at least kMinTeamStages and the
+// stages of one work unit, and no more than the shared memory left after W, slabs and bias holds.
+// Not deeper: the producer claims units as far ahead as its stages reach, and units claimed early
+// by one CTA cannot go to another, which on launches with few units per CTA undoes the dynamic
+// schedule.
+constexpr int kTeamInFlightBytes = 32 * 1024;
+constexpr int kMinTeamStages = 4;
+constexpr int kMaxStages = 3 * 16;   // mbarrier storage: three consumers of 16 stages
+constexpr int kRing = 4;          // work-unit ring entries (power of two)
 constexpr int kSmemLimit = 227 * 1024;                   // one CTA per SM
 // Weights of at most this many (padded, swizzled) bytes stay in shared memory for the life of the
 // CTA: every D0 layer up to blocks_8, the BiFPN layers and both predict layers (the class head,
 // 9 anchors x 96 x 64 halves, is exactly this size).  What is left still holds the staging slabs
 // and at least two A stages per consumer.
 constexpr int kResidentWBytes = 108 * 1024;
+constexpr int kUnitsPerCta = 8;                  // work-unit size policy (run())
+constexpr int kMaxUnitBytes = 128 * 1024;
 
 struct Params {
   int batch, rows, k, nout, nout_pad8;
@@ -60,7 +72,12 @@ struct Params {
   int desc_sbo;       // byte distance between 8-row groups in smem (8 * row pitch)
   int desc_layout;    // wgmma layout type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
   int wbatch, ldr;
-  int total_tiles;
+  // Work unit: unit_m consecutive M blocks of one image (the last unit of an image may be
+  // shorter) x one N tile, or x every N tile when hold_a is set.  One tile-ring entry and one
+  // scheduler claim cover the whole unit.
+  int unit_m, units_per_image;
+  int hold_a;         // 1: W resident, one k-block, several N tiles: A is loaded once per M block
+  int total_units;
   int bias_floats;    // floats of the zero-padded bias staged in shared memory: whole N tiles
   const float* bias;
   const __half* residual;
@@ -78,19 +95,21 @@ struct TileCoord {
 };
 constexpr int kMaxBiasSmem = 8192;
 
-__device__ __forceinline__ TileCoord decode_tile(int t, const Params& p) {
+// Work unit u -> batch entry, first M block, N tile (the first one when the unit holds A).
+__device__ __forceinline__ TileCoord decode_unit(int u, const Params& p) {
   TileCoord c;
   c.n_blk = 0;
-  if (p.num_n_blocks != 1) {       // (uniform) most layers are one N tile wide ...
-    c.n_blk = t % p.num_n_blocks;
-    t /= p.num_n_blocks;
+  if (p.num_n_blocks != 1 && !p.hold_a) {   // (uniform) most layers are one N tile wide ...
+    c.n_blk = u % p.num_n_blocks;
+    u /= p.num_n_blocks;
   }
-  c.m_blk = t;
+  c.m_blk = u;
   c.b = 0;
   if (p.batch != 1) {              // ... and one batch entry long: no division at all
-    c.m_blk = t % p.num_m_blocks;
-    c.b = t / p.num_m_blocks;
+    c.m_blk = u % p.units_per_image;
+    c.b = u / p.units_per_image;
   }
+  c.m_blk *= p.unit_m;
   return c;
 }
 
@@ -131,14 +150,14 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_bias + p.bias_floats);
   uint64_t* full_bar = bars;                       // [kMaxStages]
   uint64_t* empty_bar = bars + kMaxStages;         // [kMaxStages]
-  // Tile indices travel from the producer to the consumers through a small ring: CTA i owns tile
-  // i, every further tile comes from a global counter (sched_next_tile), so a CTA that gets its
+  // Work-unit indices travel from the producer to the consumers through a small ring: CTA i owns
+  // unit i, every further unit comes from a global counter (sched_claim), so a CTA that gets its
   // SM late -- another stream's kernel, e.g. the NMS of the previous batch, was holding it --
   // simply finds less work instead of owning a full static share.
   uint64_t* ring_full = bars + 2 * kMaxStages;     // [kRing] producer -> consumers
   uint64_t* ring_empty = ring_full + kRing;        // [kRing] consumers -> producer
-  // [kRing] x {tile, batch entry, M block, N block}: the producer decodes each tile once (its two
-  // integer divisions) and the consumers read the coordinates with one 16-byte load
+  // [kRing] x {unit, batch entry, first M block, N block}: the producer decodes each unit once
+  // (its two integer divisions) and the consumers read the coordinates with one 16-byte load
   uint64_t* w_full = ring_empty + kRing;          // [2]: [0] resident W landed, [1] padding
   volatile int4* tile_ring = reinterpret_cast<volatile int4*>(w_full + 2);
 
@@ -185,44 +204,45 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
       // bytes the TMA boxes of one stage deliver (the B slot may be padded to 1 KiB)
       const uint32_t tx_bytes =
           static_cast<uint32_t>(p.a_stage_bytes) + (p.w_resident ? 0u : w_box_bytes);
-      bool exhausted = false;
+      int u = blockIdx.x;   // the CTA's first unit; the grid is never larger than total_units
       for (int i = 0;; ++i) {
-        int t = p.total_tiles;
-        if (i == 0) {
-          t = blockIdx.x;
-        } else if (!exhausted) {
-          t = sched_next_tile(p.sched, p.total_tiles);
-          exhausted = t >= p.total_tiles;
-        }
+        // Claim the next unit before this one's loads: the returning atomic on the counter all
+        // CTAs share is only waited for at the end of this iteration.
+        const int next = u < p.total_units ? sched_claim(p.sched) : p.total_units;
         const int slot = i & (kRing - 1);
         mbar_wait(smem_u32(&ring_empty[slot]), (static_cast<uint32_t>(i / kRing) & 1u) ^ 1u);
         TileCoord tc;
         tc.b = tc.m_blk = tc.n_blk = 0;
-        if (t < p.total_tiles) tc = decode_tile(t, p);
-        const_cast<int4*>(tile_ring)[slot] = make_int4(t, tc.b, tc.m_blk, tc.n_blk);
+        if (u < p.total_units) tc = decode_unit(u, p);
+        const_cast<int4*>(tile_ring)[slot] = make_int4(u, tc.b, tc.m_blk, tc.n_blk);
         mbar_arrive(smem_u32(&ring_full[slot]));     // release: the entry is visible to waiters
-        if (t >= p.total_tiles) break;
+        if (u >= p.total_units) break;
         const int wb = (p.wbatch > 1) ? tc.b : 0;
         const int team = i % TEAMS;
         int stage = stage_of[team];
         uint32_t phase = static_cast<uint32_t>(phase_of[team]);
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          const int s = team * p.team_stages + stage;
-          mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
-          const uint32_t fb = smem_u32(&full_bar[s]);
-          mbar_expect_tx(fb, tx_bytes);
-          uint8_t* sa = smem + s * stage_bytes;
-          tma_load_3d(smem_u32(sa), &map_a, fb, kb * p.block_k, tc.m_blk * BLOCK_M, tc.b);
-          if (!p.w_resident)
-            tma_load_3d(smem_u32(sa + p.a_stage_bytes), &map_w, fb, kb * p.block_k,
-                        tc.n_blk * p.block_n, wb);
-          if (++stage == p.team_stages) {
-            stage = 0;
-            phase ^= 1;
+        const int m_end = min(tc.m_blk + p.unit_m, p.num_m_blocks);
+        for (int m_blk = tc.m_blk; m_blk < m_end; ++m_blk) {
+          for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+            const int s = team * p.team_stages + stage;
+            mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
+            const uint32_t fb = smem_u32(&full_bar[s]);
+            mbar_expect_tx(fb, tx_bytes);
+            uint8_t* sa = smem + s * stage_bytes;
+            tma_load_3d(smem_u32(sa), &map_a, fb, kb * p.block_k, m_blk * BLOCK_M, tc.b);
+            if (!p.w_resident)
+              tma_load_3d(smem_u32(sa + p.a_stage_bytes), &map_w, fb, kb * p.block_k,
+                          tc.n_blk * p.block_n, wb);
+            if (++stage == p.team_stages) {
+              stage = 0;
+              phase ^= 1;
+            }
           }
         }
         stage_of[team] = stage;
         phase_of[team] = static_cast<int>(phase);
+        u = next;
+        if (u >= p.total_units) sched_retire(p.sched);   // this CTA's last claim
       }
     }
   } else if (warp >= 4) {
@@ -259,145 +279,153 @@ pointwise_tc_kernel(const __grid_constant__ CUtensorMap map_a,
       e.w = __shfl_sync(0xffffffffu, e.w, 0);
       named_sync(1 + team, 128);
       if (wtid == 0) mbar_arrive(smem_u32(&ring_empty[slot]));
-      const int t = e.x;
-      if (t >= p.total_tiles) break;
-      if (iter % TEAMS != team) continue;   // another consumer's tile (and ring)
+      if (e.x >= p.total_units) break;
+      if (iter % TEAMS != team) continue;   // another consumer's unit (and ring)
+      // The unit's tiles, N tile fastest, with no handshake between them.  With hold_a the A stage
+      // of an M block serves every N tile against the resident W and is released after the last.
+      const int m_end = min(e.z + p.unit_m, p.num_m_blocks);
+      const int n_end = p.hold_a ? p.num_n_blocks : e.w + 1;
       TileCoord tc;
       tc.b = e.y;
-      tc.m_blk = e.z;
-      tc.n_blk = e.w;
-      const int n0 = tc.n_blk * p.block_n;
-      // only the columns that exist in the output are worth an epilogue (rounded up to 16); the
-      // rest of a ragged last N tile is skipped
-      const int n_valid = min(p.block_n, ((p.nout - n0 + 15) >> 4) << 4);
-      const int nt = n_valid >> 4;
-      float acc[NT][8];
+      for (tc.m_blk = e.z; tc.m_blk < m_end; ++tc.m_blk) {
+        for (tc.n_blk = e.w; tc.n_blk < n_end; ++tc.n_blk) {
+          const bool last_n = tc.n_blk + 1 == n_end;
+          const int n0 = tc.n_blk * p.block_n;
+          // only the columns that exist in the output are worth an epilogue (rounded up to 16); the
+          // rest of a ragged last N tile is skipped
+          const int n_valid = min(p.block_n, ((p.nout - n0 + 15) >> 4) << 4);
+          const int nt = n_valid >> 4;
+          float acc[NT][8];
 #pragma unroll
-      for (int j = 0; j < NT; ++j)
+          for (int j = 0; j < NT; ++j)
 #pragma unroll
-        for (int q = 0; q < 8; ++q) acc[j][q] = 0.f;
-      // One k-block of MMAs stays in flight: the stage of k-block kb - 1 is released once the
-      // MMAs of kb are issued and those of kb - 1 have completed.
-      int prev_s = -1;
-      for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-        const int s = team * p.team_stages + stage;
-        mbar_wait(smem_u32(&full_bar[s]), phase);
-        uint8_t* sa = smem + s * stage_bytes;
-        uint8_t* sb = p.w_resident
-                          ? smem_w + (tc.n_blk * p.num_k_blocks + kb) * p.b_stage_bytes
-                          : sa + p.a_stage_bytes;
-        const uint64_t da = make_smem_desc(smem_u32(sa), p.desc_sbo, p.desc_layout);
-        const uint64_t db = make_smem_desc(smem_u32(sb), p.desc_sbo, p.desc_layout);
-        const int k_rem = p.k - kb * p.block_k;
-        const int ksteps = k_rem >= p.block_k ? p.block_k / MMA_K : (k_rem + MMA_K - 1) / MMA_K;
-        wg_fence();
-        wg_mma_kblock_wide<NT>(acc, da, db, ksteps, kb == 0);
-        wg_commit();
-        wg_wait<1>();
-        if (prev_s >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_s]));   // this warp is done with it
-        }
-        prev_s = s;
-        advance();
-      }
-      wg_wait<0>();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_s]));
-      wg_fence_acc<NT>(acc);
-      const int row0 = tc.m_blk * BLOCK_M + r0;
-      if constexpr (EPI == EPI_ARGMAX) {
-        // Class head fused with the class half of pre-NMS (tf2/postprocess.py:88-156 with
-        // max_nms_inputs == 0): an N tile is ONE anchor (90 class columns + 6 pad columns whose
-        // bias is -inf).  Each logit is rounded to fp16 exactly as the storing epilogue would
-        // store it, then max / first arg-max / sigmoid as pre_nms_kernel does -> bit-identical
-        // scores and classes, without the [N, H, W, 810] logits ever reaching HBM.
-        const float* bias = smem_bias + tc.n_blk * kArgmaxCols;
-        uint32_t best[2] = {0u, 0u};                  // rows r0, r0 + 8
-#pragma unroll
-        for (int j = 0; j < kArgmaxCols / 16; ++j) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int col = 16 * j + 8 * h + cq;
-            const float2 b = *reinterpret_cast<const float2*>(bias + col);
-#pragma unroll
-            for (int r = 0; r < 2; ++r) {
-              const float2 s = fadd2_rn(make_float2(acc[j][4 * h + 2 * r], acc[j][4 * h + 2 * r + 1]), b);
-              best[r] = max(best[r], argmax_pair_key(s, static_cast<uint32_t>(col)));
+            for (int q = 0; q < 8; ++q) acc[j][q] = 0.f;
+          // One k-block of MMAs stays in flight: the stage of k-block kb - 1 is released once the
+          // MMAs of kb are issued and those of kb - 1 have completed.
+          int prev_s = -1;
+          for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+            const int s = team * p.team_stages + stage;
+            if (tc.n_blk == e.w) mbar_wait(smem_u32(&full_bar[s]), phase);
+            uint8_t* sa = smem + s * stage_bytes;
+            uint8_t* sb = p.w_resident
+                              ? smem_w + (tc.n_blk * p.num_k_blocks + kb) * p.b_stage_bytes
+                              : sa + p.a_stage_bytes;
+            const uint64_t da = make_smem_desc(smem_u32(sa), p.desc_sbo, p.desc_layout);
+            const uint64_t db = make_smem_desc(smem_u32(sb), p.desc_sbo, p.desc_layout);
+            const int k_rem = p.k - kb * p.block_k;
+            const int ksteps = k_rem >= p.block_k ? p.block_k / MMA_K : (k_rem + MMA_K - 1) / MMA_K;
+            wg_fence();
+            wg_mma_kblock_wide<NT>(acc, da, db, ksteps, kb == 0);
+            wg_commit();
+            wg_wait<1>();
+            if (prev_s >= 0) {
+              __syncwarp();
+              if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_s]));   // this warp is done with it
             }
+            prev_s = s;
+            if (last_n) advance();   // hold_a (one k-block): the stage stays for the next N tile
           }
-        }
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {      // the four lanes of a quad hold the same row
-          best[r] = max(best[r], __shfl_xor_sync(0xffffffffu, best[r], 1));
-          best[r] = max(best[r], __shfl_xor_sync(0xffffffffu, best[r], 2));
-          const uint32_t ord_best = best[r] >> 16;
-          const unsigned short hbits = static_cast<unsigned short>(
-              (ord_best & 0x8000u) ? (ord_best ^ 0x8000u) : (~ord_best & 0xFFFFu));
-          const float bv = __half2float(__ushort_as_half(hbits));
-          const int best_c = static_cast<int>(0xFFFFu - (best[r] & 0xFFFFu));
-          const int row = row0 + 8 * r;
-          if ((lane & 3) == 0 && row < p.rows) {
-            const size_t o = static_cast<size_t>(tc.b) * p.am_total + p.am_anchor_begin +
-                             static_cast<size_t>(row) * p.am_num_anchors + tc.n_blk;
-            p.am_scores[o] = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-bv)));
-            p.am_classes[o] = best_c;
+          wg_wait<0>();
+          if (last_n) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev_s]));
           }
-        }
-      } else {
-        const bool ok[2] = {row0 < p.rows, row0 + 8 < p.rows};
-        const __half* res_row[2] = {nullptr, nullptr};
-        if (HAS_RES) {
+          wg_fence_acc<NT>(acc);
+          const int row0 = tc.m_blk * BLOCK_M + r0;
+          if constexpr (EPI == EPI_ARGMAX) {
+            // Class head fused with the class half of pre-NMS (tf2/postprocess.py:88-156 with
+            // max_nms_inputs == 0): an N tile is ONE anchor (90 class columns + 6 pad columns whose
+            // bias is -inf).  Each logit is rounded to fp16 exactly as the storing epilogue would
+            // store it, then max / first arg-max / sigmoid as pre_nms_kernel does -> bit-identical
+            // scores and classes, without the [N, H, W, 810] logits ever reaching HBM.
+            const float* bias = smem_bias + tc.n_blk * kArgmaxCols;
+            uint32_t best[2] = {0u, 0u};                  // rows r0, r0 + 8
 #pragma unroll
-          for (int r = 0; r < 2; ++r)
-            res_row[r] = p.residual +
-                         (static_cast<size_t>(tc.b) * p.rows + (ok[r] ? row0 + 8 * r : 0)) * p.ldr;
-        }
-        // a slab set is free once the stores that last read it (this consumer's previous tile, or
-        // the one before that with two sets) have read it
-        uint8_t* my_slabs = team_slabs + (my_tiles % p.slab_sets) * p.slab_set_bytes;
-        ++my_tiles;
-        if (wtid == 0) {
-          if (p.slab_sets == 2)
-            tma_store_wait_read<1>();
-          else
-            tma_store_wait_read<0>();
-        }
-        named_sync(1 + team, 128);
+            for (int j = 0; j < kArgmaxCols / 16; ++j) {
 #pragma unroll
-        for (int j = 0; j < NT; ++j) {
-          if (j < nt) {
-            const int colt = 16 * j + cq;            // tile column of acc[j][0]
-            const float2 b_lo = *reinterpret_cast<const float2*>(smem_bias + n0 + colt);
-            const float2 b_hi = *reinterpret_cast<const float2*>(smem_bias + n0 + colt + 8);
-            uint8_t* slab = my_slabs + (colt >> 6) * kSlabBytes;
-            const int piece = (colt & 63) >> 3;      // 16-byte piece of the 128-byte slab row
+              for (int h = 0; h < 2; ++h) {
+                const int col = 16 * j + 8 * h + cq;
+                const float2 b = *reinterpret_cast<const float2*>(bias + col);
 #pragma unroll
-            for (int r = 0; r < 2; ++r) {
-              float2 lo = fadd2_rn(make_float2(acc[j][2 * r], acc[j][2 * r + 1]), b_lo);
-              float2 hi = fadd2_rn(make_float2(acc[j][4 + 2 * r], acc[j][4 + 2 * r + 1]), b_hi);
-              apply_act4<ACT>(lo, hi);
-              if (HAS_RES && ok[r]) {
-                const int col = n0 + colt;
-                if (col < p.nout)
-                  lo = fadd2_rn(lo, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col)));
-                if (col + 8 < p.nout)
-                  hi = fadd2_rn(hi, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col + 8)));
+                for (int r = 0; r < 2; ++r) {
+                  const float2 s = fadd2_rn(make_float2(acc[j][4 * h + 2 * r], acc[j][4 * h + 2 * r + 1]), b);
+                  best[r] = max(best[r], argmax_pair_key(s, static_cast<uint32_t>(col)));
+                }
               }
-              const int row = r0 + 8 * r;
-              uint8_t* rb = slab + row * 128 + cq * 2;
-              *reinterpret_cast<__half2*>(rb + ((piece ^ (row & 7)) << 4)) = __floats2half2_rn(lo.x, lo.y);
-              *reinterpret_cast<__half2*>(rb + (((piece + 1) ^ (row & 7)) << 4)) = __floats2half2_rn(hi.x, hi.y);
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {      // the four lanes of a quad hold the same row
+              best[r] = max(best[r], __shfl_xor_sync(0xffffffffu, best[r], 1));
+              best[r] = max(best[r], __shfl_xor_sync(0xffffffffu, best[r], 2));
+              const uint32_t ord_best = best[r] >> 16;
+              const unsigned short hbits = static_cast<unsigned short>(
+                  (ord_best & 0x8000u) ? (ord_best ^ 0x8000u) : (~ord_best & 0xFFFFu));
+              const float bv = __half2float(__ushort_as_half(hbits));
+              const int best_c = static_cast<int>(0xFFFFu - (best[r] & 0xFFFFu));
+              const int row = row0 + 8 * r;
+              if ((lane & 3) == 0 && row < p.rows) {
+                const size_t o = static_cast<size_t>(tc.b) * p.am_total + p.am_anchor_begin +
+                                 static_cast<size_t>(row) * p.am_num_anchors + tc.n_blk;
+                p.am_scores[o] = __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-bv)));
+                p.am_classes[o] = best_c;
+              }
+            }
+          } else {
+            const bool ok[2] = {row0 < p.rows, row0 + 8 < p.rows};
+            const __half* res_row[2] = {nullptr, nullptr};
+            if (HAS_RES) {
+#pragma unroll
+              for (int r = 0; r < 2; ++r)
+                res_row[r] = p.residual +
+                             (static_cast<size_t>(tc.b) * p.rows + (ok[r] ? row0 + 8 * r : 0)) * p.ldr;
+            }
+            // a slab set is free once the stores that last read it (this consumer's previous tile, or
+            // the one before that with two sets) have read it
+            uint8_t* my_slabs = team_slabs + (my_tiles % p.slab_sets) * p.slab_set_bytes;
+            ++my_tiles;
+            if (wtid == 0) {
+              if (p.slab_sets == 2)
+                tma_store_wait_read<1>();
+              else
+                tma_store_wait_read<0>();
+            }
+            named_sync(1 + team, 128);
+#pragma unroll
+            for (int j = 0; j < NT; ++j) {
+              if (j < nt) {
+                const int colt = 16 * j + cq;            // tile column of acc[j][0]
+                const float2 b_lo = *reinterpret_cast<const float2*>(smem_bias + n0 + colt);
+                const float2 b_hi = *reinterpret_cast<const float2*>(smem_bias + n0 + colt + 8);
+                uint8_t* slab = my_slabs + (colt >> 6) * kSlabBytes;
+                const int piece = (colt & 63) >> 3;      // 16-byte piece of the 128-byte slab row
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                  float2 lo = fadd2_rn(make_float2(acc[j][2 * r], acc[j][2 * r + 1]), b_lo);
+                  float2 hi = fadd2_rn(make_float2(acc[j][4 + 2 * r], acc[j][4 + 2 * r + 1]), b_hi);
+                  apply_act4<ACT>(lo, hi);
+                  if (HAS_RES && ok[r]) {
+                    const int col = n0 + colt;
+                    if (col < p.nout)
+                      lo = fadd2_rn(lo, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col)));
+                    if (col + 8 < p.nout)
+                      hi = fadd2_rn(hi, __half22float2(*reinterpret_cast<const __half2*>(res_row[r] + col + 8)));
+                  }
+                  const int row = r0 + 8 * r;
+                  uint8_t* rb = slab + row * 128 + cq * 2;
+                  *reinterpret_cast<__half2*>(rb + ((piece ^ (row & 7)) << 4)) = __floats2half2_rn(lo.x, lo.y);
+                  *reinterpret_cast<__half2*>(rb + (((piece + 1) ^ (row & 7)) << 4)) = __floats2half2_rn(hi.x, hi.y);
+                }
+              }
+            }
+            fence_proxy_async_smem();
+            named_sync(1 + team, 128);
+            if (wtid == 0) {
+              for (int c = 0; c * kStoreCols < n_valid; ++c)
+                tma_store_3d(&map_o, smem_u32(my_slabs + c * kSlabBytes), n0 + c * kStoreCols,
+                             tc.m_blk * BLOCK_M, tc.b);
+              tma_store_commit();
             }
           }
-        }
-        fence_proxy_async_smem();
-        named_sync(1 + team, 128);
-        if (wtid == 0) {
-          for (int c = 0; c * kStoreCols < n_valid; ++c)
-            tma_store_3d(&map_o, smem_u32(my_slabs + c * kSlabBytes), n0 + c * kStoreCols,
-                         tc.m_blk * BLOCK_M, tc.b);
-          tma_store_commit();
         }
       }
     }
@@ -466,7 +494,6 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   p.ldr = ldr;
   p.bias = bias;
   p.residual = residual;
-  p.total_tiles = batch * p.num_m_blocks * p.num_n_blocks;
   p.sched = next_sched_slot();
   if (!p.sched) return EDET_ERR_CUDA;
 
@@ -486,6 +513,7 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   const int w_bytes = p.num_n_blocks * p.num_k_blocks * p.b_stage_bytes;
   p.w_resident = wbatch == 1 && w_bytes <= kResidentWBytes;
   p.stage_bytes = p.a_stage_bytes + (p.w_resident ? 0 : p.b_stage_bytes);
+
   // the arg-max epilogue stores nothing through TMA: no staging slabs
   p.slab_set_bytes = am ? 0 : ceil_div(p.block_n, kStoreCols) * kSlabBytes;
   const int opt_kb = option_pw_smem_kb();
@@ -498,12 +526,46 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   // that still leaves each consumer three stages; else one.
   p.slab_sets = (limit - 1024 - fixed_bytes(2)) / p.stage_bytes >= 3 * teams ? 2 : 1;
   const int fixed = fixed_bytes(p.slab_sets);
-  int stages = (limit - 1024 - fixed) / p.stage_bytes;
-  if (stages > kMaxStages) stages = kMaxStages;
-  p.team_stages = stages / teams;            // each consumer's own ring
-  EDET_CHECK_ARG(p.team_stages >= 2, "pointwise_tc: block_n %d leaves <2 pipeline stages per consumer",
+  // the most stages each consumer's own ring can have
+  const int max_team_stages =
+      std::min((limit - 1024 - fixed) / p.stage_bytes, kMaxStages) / teams;
+  EDET_CHECK_ARG(max_team_stages >= 2, "pointwise_tc: block_n %d leaves <2 pipeline stages per consumer",
                  p.block_n);
-  stages = p.team_stages * teams;
+
+  const int sm_count = device_sm_count();
+  if (!sm_count) return EDET_ERR_CUDA;
+  int grid = sm_count - option_persist_slack();
+  if (grid < 1) grid = 1;
+  // Work units.  With W resident and one k-block an M block's A tile serves every N tile (the
+  // class head: all anchors of its rows).  A is held only while the M blocks alone still give
+  // every CTA a unit: with fewer (the small class-head levels) the N tiles of an M block finish
+  // sooner spread over several CTAs.
+  p.hold_a = p.w_resident && p.num_n_blocks > 1 && p.num_k_blocks == 1 &&
+             batch * p.num_m_blocks >= grid;
+  const int unit_n_blocks = p.hold_a ? p.num_n_blocks : 1;
+  // bytes of one M block of a unit: its stages (A, and W when streamed) and its output tiles
+  const int m_block_bytes =
+      p.num_k_blocks * p.stage_bytes + unit_n_blocks * BLOCK_M * p.block_n * 2;
+  auto units_for = [&](int g) {
+    return batch * ceil_div(p.num_m_blocks, g) * (p.hold_a ? 1 : p.num_n_blocks);
+  };
+  // A unit is the largest of 1, 2, 4, 8 M blocks that still leaves at least kUnitsPerCta units
+  // per CTA (the tail of the dynamic schedule stays short), moves at most kMaxUnitBytes, and whose
+  // stages fit in one consumer's ring (the single producer fills the consumers' rings in unit
+  // order, so a unit that does not fit would keep the other consumer waiting).  The per-unit
+  // handshake and claim are then spread over several tiles.
+  p.unit_m = 8;
+  while (p.unit_m > 1 && (units_for(p.unit_m) < kUnitsPerCta * grid ||
+                          p.unit_m * m_block_bytes > kMaxUnitBytes ||
+                          p.unit_m * p.num_k_blocks > max_team_stages))
+    p.unit_m >>= 1;
+  p.units_per_image = ceil_div(p.num_m_blocks, p.unit_m);
+  p.total_units = units_for(p.unit_m);
+  if (p.total_units < grid) grid = p.total_units;
+  p.team_stages = std::min(max_team_stages,
+                           std::max({kMinTeamStages, ceil_div(kTeamInFlightBytes, p.stage_bytes),
+                                     p.unit_m * p.num_k_blocks}));
+  const int stages = p.team_stages * teams;
   p.num_stages = stages;
   p.desc_layout = desc_layout_for(p.block_k);
   p.desc_sbo = 8 * p.block_k * 2;
@@ -525,11 +587,6 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
     return rc;
   }
 
-  const int sm_count = device_sm_count();
-  if (!sm_count) return EDET_ERR_CUDA;
-  int grid = sm_count - option_persist_slack();
-  if (grid < 1) grid = 1;
-  if (p.total_tiles < grid) grid = p.total_tiles;
   const bool has_res = residual != nullptr;
   if (am) return launch<EDET_ACT_NONE, false, 2, EPI_ARGMAX>(ma, mw, mo, p, grid, smem_bytes, stream);
 

@@ -277,16 +277,23 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map
 // tile i and every further tile comes from a global counter, so late CTAs simply find less (or
 // no) work.  sched[0] = tiles handed out beyond the first gridDim.x, sched[1] = CTAs that are
 // done; the last CTA resets both, so a slot is reusable by the next launch without a memset.
-__device__ __forceinline__ int sched_next_tile(unsigned* sched, int total_tiles) {
-  const int t = static_cast<int>(gridDim.x + atomicAdd(&sched[0], 1u));
-  if (t >= total_tiles) {     // this CTA's last fetch
+// A CTA stops claiming after its first claim >= total_tiles and then calls sched_retire once.
+// sched_claim does not look at its result, so a caller can issue it ahead of other work and only
+// wait for the atomic where it uses the tile.
+__device__ __forceinline__ int sched_claim(unsigned* sched) {
+  return static_cast<int>(gridDim.x + atomicAdd(&sched[0], 1u));
+}
+__device__ __forceinline__ void sched_retire(unsigned* sched) {
+  __threadfence();
+  if (atomicAdd(&sched[1], 1u) == gridDim.x - 1) {
+    sched[0] = 0u;
+    sched[1] = 0u;
     __threadfence();
-    if (atomicAdd(&sched[1], 1u) == gridDim.x - 1) {
-      sched[0] = 0u;
-      sched[1] = 0u;
-      __threadfence();
-    }
   }
+}
+__device__ __forceinline__ int sched_next_tile(unsigned* sched, int total_tiles) {
+  const int t = sched_claim(sched);
+  if (t >= total_tiles) sched_retire(sched);   // this CTA's last fetch
   return t;
 }
 // Pool of self-resetting scheduler counters, one pool per device (defined in capi.cu).
