@@ -484,9 +484,10 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   p.nout = nout;
   p.nout_pad8 = nout & ~7;   // whole float4 pairs of bias that are in bounds
   // Consumer warpgroups: two by default (one in its epilogue while the other one's MMAs run);
-  // edet_set_option("pw_teams", 2 | 3) forces a variant for A/B measurements.
+  // edet_set_option("pw_teams", 2 | 3) forces a variant for A/B measurements.  The arg-max
+  // epilogue is only instantiated with two, so its rings are planned for two.
   const int opt_teams = option_pw_teams();
-  const int teams = opt_teams ? opt_teams : 2;
+  const int teams = (opt_teams && !am) ? opt_teams : 2;
   p.block_n = am ? kArgmaxCols : pick_block_n(nout);
   p.num_m_blocks = ceil_div(rows, BLOCK_M);
   p.num_n_blocks = ceil_div(nout, p.block_n);
@@ -512,7 +513,6 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   // (SE-scaled) weights keep streaming with A.
   const int w_bytes = p.num_n_blocks * p.num_k_blocks * p.b_stage_bytes;
   p.w_resident = wbatch == 1 && w_bytes <= kResidentWBytes;
-  p.stage_bytes = p.a_stage_bytes + (p.w_resident ? 0 : p.b_stage_bytes);
 
   // the arg-max epilogue stores nothing through TMA: no staging slabs
   p.slab_set_bytes = am ? 0 : ceil_div(p.block_n, kStoreCols) * kSlabBytes;
@@ -522,6 +522,12 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
     return (p.w_resident ? w_bytes : 0) + teams * sets * p.slab_set_bytes + p.bias_floats * 4 +
            (2 * kMaxStages + 2 * kRing + 2) * 8 + 16 * kRing;
   };
+  // Under a smaller pw_smem_kb budget resident W may not leave two A stages per consumer next to
+  // one slab set: W then streams with A.  At the default budget every W of at most
+  // kResidentWBytes leaves that room, so this only changes plans that would otherwise be refused.
+  if (p.w_resident && (limit - 1024 - fixed_bytes(1)) / p.a_stage_bytes < 2 * teams)
+    p.w_resident = 0;
+  p.stage_bytes = p.a_stage_bytes + (p.w_resident ? 0 : p.b_stage_bytes);
   // Two slab sets per consumer (the stores of one tile drain while the next epilogue writes) when
   // that still leaves each consumer three stages; else one.
   p.slab_sets = (limit - 1024 - fixed_bytes(2)) / p.stage_bytes >= 3 * teams ? 2 : 1;

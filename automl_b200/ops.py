@@ -180,13 +180,14 @@ CLASS_ARGMAX_COLS = 96   # columns per anchor of the padded class-head weights (
 
 def class_argmax(a, wt_padded, bias_padded, scores, classes, anchor_begin, num_anchors):
   """Class-predict 1x1 conv fused with the class half of pre-NMS for one level: a fp16
-  [N,H,W,F] (the depthwise output of the predict layer), wt_padded fp16 [num_anchors*96, F] (row
-  a*96 + c = class c of anchor a, zero rows for c >= num_classes), bias_padded fp32
-  [num_anchors*96] (-inf on the pad rows) -> scores fp32 / classes i32 [N, total_anchors] at
-  anchors anchor_begin + pixel*num_anchors + a."""
-  n, h, w, f = a.shape
-  assert wt_padded.shape == (num_anchors * CLASS_ARGMAX_COLS, f)
-  _lib.call('edet_class_argmax', _ptr(a, torch.float16), f, _ptr(wt_padded, torch.float16),
+  [N,H,W,lda] (the depthwise output of the predict layer, F = wt_padded.shape[-1] <= lda
+  channels), wt_padded fp16 [num_anchors*96, F] (row a*96 + c = class c of anchor a, zero rows
+  for c >= num_classes), bias_padded fp32 [num_anchors*96] (-inf on the pad rows) -> scores fp32 /
+  classes i32 [N, total_anchors] at anchors anchor_begin + pixel*num_anchors + a."""
+  n, h, w, lda = a.shape
+  f = wt_padded.shape[-1]
+  assert wt_padded.shape == (num_anchors * CLASS_ARGMAX_COLS, f) and f <= lda
+  _lib.call('edet_class_argmax', _ptr(a, torch.float16), lda, _ptr(wt_padded, torch.float16),
             _ptr(bias_padded, torch.float32), _ptr(scores, torch.float32),
             _ptr(classes, torch.int32), anchor_begin, scores.shape[1], num_anchors, n, h * w, f,
             _stream())

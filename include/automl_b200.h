@@ -62,7 +62,10 @@ const char* edet_last_error(void);
  * two consumer warpgroups) | 2 | 3; "stem_impl" = 0 (default: tensor-core stem) | 1 (CUDA-core stem);
  * "sepconv_impl" = 0 (default: TMA-staged input tile for c <= 64, one buffer, four CTAs per SM) |
  * 1 (loads from global) | 2 (TMA, two buffers, three CTAs per SM);
- * "pw_smem_kb" = 0 (default: 227 KiB, one pointwise CTA per SM) | 64..227;
+ * "pw_smem_kb" = 0 (default: 227 KiB, one pointwise CTA per SM) | 64..227: every shape runs from
+ * 162 KiB up with two consumers and from 226 KiB with three (the widest plan: 128 x 64 W tiles
+ * streamed with A, nout 8192); a smaller budget refuses the shapes it cannot hold with
+ * EDET_ERR_INVALID;
  * "persist_slack" = CTAs a persistent kernel leaves out of its grid (default 0). */
 int edet_set_option(const char* name, int value);
 int edet_get_option(const char* name, int* value);

@@ -26,8 +26,11 @@ def rel_l2(a, b):
 
 
 def act_ref(x, act):
+  # float64 forms of utils.py's activation_fn
   return {utils.ACT_NONE: lambda t: t, utils.ACT_SWISH: lambda t: t * torch.sigmoid(t),
-          utils.ACT_RELU6: lambda t: torch.clamp(t, 0, 6)}[act](x)
+          utils.ACT_RELU: torch.relu, utils.ACT_RELU6: lambda t: torch.clamp(t, 0, 6),
+          utils.ACT_HSWISH: lambda t: t * torch.clamp(t + 3, 0, 6) / 6,
+          utils.ACT_SIGMOID: torch.sigmoid}[act](x)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -52,7 +55,21 @@ PW_CASES = [
     (1, 513, 256, 256, utils.ACT_SWISH, True, False),
     (1, 900, 384, 384, utils.ACT_NONE, False, False),        # N > 256: tiles of 96 columns
     (1, 260, 1344, 224, utils.ACT_NONE, True, True),        # D4-sized project
+    # the other activations of utils.activation_fn, with a bias (_act_bias) that spreads the
+    # pre-activations over every kink (-3, 0, 3, 6) and below -21, where the swish clamp acts
+    (1, 1000, 64, 96, utils.ACT_RELU, False, False, 'span'),
+    (2, 700, 40, 200, utils.ACT_HSWISH, True, False, 'span'),      # two N tiles + residual
+    (1, 900, 16, 64, utils.ACT_SIGMOID, False, False, 'span'),
+    (1, 800, 96, 128, utils.ACT_SWISH, False, False, 'span'),
+    (2, 300, 672, 112, utils.ACT_HSWISH, False, True, 'span'),     # streamed per-image W
 ]
+
+
+def _act_bias(nout, g, span):
+  """Column biases: N(0, 1), or with `span` evenly over [-26, 10] (the GEMM part is ~N(0, 1))."""
+  if not span:
+    return torch.randn(nout, generator=g)
+  return torch.linspace(-26.0, 10.0, nout)[torch.randperm(nout, generator=g)]
 
 
 @pytest.mark.parametrize('impl_name', ['tcgen05', 'simt'])
@@ -60,12 +77,12 @@ PW_CASES = [
 def test_pointwise_conv(case, impl_name):
   ops = _ops()
   impl = ops.PW_TCGEN05 if impl_name == 'tcgen05' else ops.PW_SIMT
-  batch, rows, k, nout, act, has_res, per_image = case
+  batch, rows, k, nout, act, has_res, per_image = case[:7]
   g = torch.Generator().manual_seed(1234 + rows + k + nout)
   a = torch.randn(batch, rows, k, generator=g).half()
   wb = batch if per_image else 1
   w = (torch.randn(wb, nout, k, generator=g) / np.sqrt(k)).half()
-  bias = torch.randn(nout, generator=g)
+  bias = _act_bias(nout, g, len(case) > 7)
   ldo = (nout + 7) // 8 * 8
   res = torch.randn(batch, rows, ldo, generator=g).half() if has_res else None
   out = torch.full((batch, rows, ldo), 7.0).half().to(DEV)
@@ -101,12 +118,12 @@ def test_pointwise_epilogue_teams_agree(case):
   turn, each with its own stage ring) do the same MMAs and the same fp32 epilogue arithmetic:
   bit-identical outputs."""
   ops = _ops()
-  batch, rows, k, nout, act, has_res, per_image = case
+  batch, rows, k, nout, act, has_res, per_image = case[:7]
   g = torch.Generator().manual_seed(4321 + rows + k + nout)
   a = torch.randn(batch, rows, k, generator=g).half().to(DEV)
   wb = batch if per_image else 1
   w = (torch.randn(wb, nout, k, generator=g) / np.sqrt(k)).half().to(DEV)
-  bias = torch.randn(nout, generator=g).to(DEV)
+  bias = _act_bias(nout, g, len(case) > 7).to(DEV)
   ldo = -(-nout // 8) * 8
   res = torch.randn(batch, rows, ldo, generator=g).half().to(DEV) if has_res else None
   outs = []
@@ -142,16 +159,19 @@ DW_CASES = [
     (1, 5, 5, 64, 3, 1, utils.ACT_NONE, False, False),
     (1, 64, 64, 1152, 5, 1, utils.ACT_SWISH, True, True),
     (1, 12, 12, 672, 5, 2, utils.ACT_RELU6, True, False),
-    # maps large enough for the TMA-tiled kernel (depthwise_tile.cu): ragged tiles in x and y,
-    # channel counts that are not multiples of the 64-channel slice, every (k, stride)
-    (2, 50, 70, 144, 3, 1, utils.ACT_SWISH, True, True),
+    # maps large enough for the TMA-tiled kernel (depthwise_tile.cu, dwt::eligible): ragged tiles
+    # in x and y, channel counts that are not multiples of the 64-channel slice, every (k, stride)
+    (2, 50, 70, 144, 3, 1, utils.ACT_SWISH, True, True),    # register kernel: 16 x 16 tiles waste
+                                                            # > 30 % (the tiled k3s1 case is below)
     (1, 67, 45, 240, 5, 1, utils.ACT_SWISH, True, True),
     (2, 61, 83, 96, 3, 2, utils.ACT_SWISH, True, True),
     (1, 97, 59, 144, 5, 2, utils.ACT_SWISH, True, True),
     (3, 48, 48, 64, 3, 1, utils.ACT_NONE, False, False),    # head depthwise at level 3 size
     (1, 80, 80, 672, 5, 1, utils.ACT_RELU6, True, True),
     (1, 160, 160, 72, 5, 2, utils.ACT_RELU6, True, False),  # c % 16 != 0
-    (2, 33, 200, 480, 3, 1, utils.ACT_NONE, True, False),   # many work units per CTA (ring wrap)
+    (2, 33, 200, 480, 3, 1, utils.ACT_NONE, True, False),   # register kernel (> 30 % waste)
+    (2, 50, 62, 144, 3, 1, utils.ACT_SWISH, True, True),    # tiled k3s1, ragged in x and y
+    (2, 49, 200, 480, 3, 1, utils.ACT_NONE, True, False),   # tiled, 832 work units (ring wrap)
 ]
 
 
