@@ -45,7 +45,10 @@ SIGNATURES = {
                                     c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'edet_conv2d': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                             c_int, c_int, c_int, c_int, c_int, c_void_p]),
-    'edet_mbconv_expand_dw': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+    'edet_conv2d_transpose': (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
+                                      c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                      c_void_p]),
+    'edet_mbconv_expand_dw':(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
                                       c_int, c_void_p]),
     'edet_se_fc': (c_int, [c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

@@ -40,6 +40,51 @@ NodeSpec = collections.namedtuple('NodeSpec', [
 ])
 
 
+HEADS = ('object_detection', 'segmentation')
+
+# One Conv2DTranspose 3x3 stride 2 'SAME' of the segmentation head
+# (tf2/efficientdet_keras.py:676-706): max_level - min_level stages (+ BN + act, then the concat
+# with the next finer BiFPN level), then the final layer (bias, no BN / act).
+SegStageSpec = collections.namedtuple('SegStageSpec', [
+    'kernel_scope',  # 'segmentation_head/conv2d_transpose[_i]'
+    'bn_scope',      # 'segmentation_head/bn_<i>', None for the final layer
+    'in_hw', 'out_hw',
+    'in_channels',   # F for the first stage, 2F (x, skip) after it
+    'out_channels',  # F, seg_num_classes for the final layer
+    'skip_level',    # BiFPN level concatenated after the stage, None for the final layer
+])
+
+
+def _seg_stages(arch):
+  """Layer list of SegmentationHead for a resolved architecture.  Variable names follow Keras'
+  default layer naming in a fresh model (the unnamed Conv2DTranspose layers become
+  conv2d_transpose, conv2d_transpose_1, ... in creation order, the head's own last); they cannot
+  be checked against a real checkpoint offline."""
+  f = arch.fpn_filters
+  stages = []
+  n = arch.max_level - arch.min_level
+  for i in range(n + 1):
+    level = arch.max_level - i
+    in_hw = arch.level_hw[level] if i == 0 else stages[-1].out_hw
+    out_hw = (2 * in_hw[0], 2 * in_hw[1])
+    final = i == n
+    if not final and out_hw != arch.level_hw[level - 1]:
+      # the reference's tf.concat (efficientdet_keras.py:703) fails on these shapes
+      raise ValueError(
+          'segmentation head: P{} is {}x{}, upsampled to {}x{}, but P{} is {}x{}; every level '
+          'must be exactly twice the next one (image size {})'.format(
+              level, in_hw[0], in_hw[1], out_hw[0], out_hw[1], level - 1,
+              arch.level_hw[level - 1][0], arch.level_hw[level - 1][1], arch.image_hw))
+    stages.append(SegStageSpec(
+        kernel_scope='segmentation_head/conv2d_transpose' + ('_%d' % i if i else ''),
+        bn_scope=None if final else 'segmentation_head/bn_%d' % i,
+        in_hw=in_hw, out_hw=out_hw,
+        in_channels=f if i == 0 else 2 * f,
+        out_channels=arch.config.seg_num_classes if final else f,
+        skip_level=None if final else level - 1))
+  return stages
+
+
 def _resample_mode(in_hw, out_hw):
   (h, w), (th, tw) = in_hw, out_hw
   if h > th and w > tw:
@@ -67,6 +112,7 @@ class DetArch(object):
     if p.backbone_config is not None:
       raise NotImplementedError('custom backbone_config')
     self.config = p
+    self._resolve_heads(p)
     self.act_type = p.act_type
     self.image_hw = utils.parse_image_size(p.image_size)
     self.min_level, self.max_level = p.min_level, p.max_level
@@ -181,6 +227,25 @@ class DetArch(object):
       self.cells.append({'nodes': nodes, 'out_index': out_idx})
       feats = [(l, self.fpn_filters)
                for l in range(p.min_level, p.max_level + 1)]
+
+    # ---- segmentation head -------------------------------------------------------
+    self.seg_stages = _seg_stages(self) if self.has_segmentation else []
+
+  def _resolve_heads(self, p):
+    """config.heads: a non-empty subset of HEADS (tf2/efficientdet_keras.py:842-884; anything else
+    builds no head in the reference and train_lib.py:637 raises)."""
+    heads = p.get('heads', None)
+    heads = ['object_detection'] if heads is None else list(heads)
+    if not heads or any(h not in HEADS for h in heads):
+      raise ValueError('No valid head found: {}'.format(heads))
+    self.heads = heads
+    self.has_detection = 'object_detection' in heads
+    self.has_segmentation = 'segmentation' in heads
+    if self.has_segmentation and p.data_format == 'channels_first':
+      # tf2/efficientdet_keras.py:703 concatenates on axis -1, the WIDTH axis in NCHW
+      raise NotImplementedError(
+          'segmentation head with channels_first: the reference concatenates on axis -1, '
+          'which is a width concat there, not a channel concat')
 
   # -- convenience ---------------------------------------------------------------
   @property

@@ -68,10 +68,21 @@ def get_engine(config, batch_size, weights=None, device='cuda:0', **engine_kwarg
   return eng
 
 
+def _detection_only(config):
+  """The legacy graph (efficientdet_arch.py:547-577) builds the class / box nets whatever
+  config.heads says and has no segmentation head (that one is EfficientDetNet's,
+  automl_b200/efficientdet_keras.py)."""
+  if list(config.get('heads', None) or ['object_detection']) == ['object_detection']:
+    return config
+  config = hparams_config.Config(config.as_dict())
+  config.heads = ['object_detection']
+  return config
+
+
 def efficientdet(features, model_name=None, config=None, weights=None, device='cuda:0',
                  **kwargs):
   """Build + run the EfficientDet network; see module docstring."""
-  config = resolve_config(model_name, config, **kwargs)
+  config = _detection_only(resolve_config(model_name, config, **kwargs))
   x = torch.as_tensor(features)
   if config.data_format == 'channels_first':
     x = x.permute(0, 2, 3, 1)

@@ -402,7 +402,9 @@ class Engine(object):
     self.fuse_class_argmax = bool(self.fuse_class_argmax and not int(nms_cfg.get('max_nms_inputs', 0) or 0)
                                   and C <= ops.CLASS_ARGMAX_COLS and self.pw_impl == ops.PW_TCGEN05)
     anchor_begin = 0
-    for net, pred_c, ld in (('class', A * C, self.ld_cls), ('box', A * 4, self.ld_box)):
+    towers = ((('class', A * C, self.ld_cls), ('box', A * 4, self.ld_box))
+              if a.has_detection else ())
+    for net, pred_c, ld in towers:
       scope = '%s_net' % net
       dws, pws, pbs = [], [], []
       for i in range(a.head_repeats):
@@ -474,6 +476,7 @@ class Engine(object):
           anchor_begin += hh * ww * A
         (self.cls_out if net == 'class' else self.box_out)[level] = out
     self._branch = None
+    self._build_segmentation(w)
     self.num_network_ops = len(self._ops)
 
     # -- post-processing ----------------------------------------------------------------------
@@ -492,11 +495,12 @@ class Engine(object):
     # Two sets of post-processing buffers: NMS of step i runs on its own stream while the
     # network of step i+1 (which writes the OTHER set) already runs on the main stream.
     self._post = []
-    cls_l = [self.cls_out[l] for l in a.levels]
-    box_l = [self.box_out[l] for l in a.levels]
+    cls_l = [self.cls_out[l] for l in a.levels if l in self.cls_out]
+    box_l = [self.box_out[l] for l in a.levels if l in self.box_out]
     level_hw = [a.level_hw[l] for l in a.levels]
     self._pre_ops, self._nms_ops, self._pre_ops_full = [], [], []
-    for sidx in range(2):
+    # no object_detection head: no pre-NMS / NMS buffers or launches (detect() raises)
+    for sidx in range(2 if a.has_detection else 0):
       ps = {
           'boxes': self._buf('boxes%d' % sidx, (n, K, 4), f32),
           'scores': self._buf('scores%d' % sidx, (n, K), f32),
@@ -556,9 +560,47 @@ class Engine(object):
       pre_bytes = 2 * sum(t.numel() for t in box_l) + 16 * n * K + 16 * K
     else:
       pre_bytes = 2 * sum(t.numel() for t in cls_l + box_l) + 24 * n * K + 16 * K
-    self._add('pre_nms', self._pre_ops[0], kind='pre_nms', nbytes=pre_bytes)
-    self._add('nms', self._nms_ops[0], kind='nms_v5', nbytes=28 * n * K, kernels=2)
+    if a.has_detection:
+      self._add('pre_nms', self._pre_ops[0], kind='pre_nms', nbytes=pre_bytes)
+      self._add('nms', self._nms_ops[0], kind='nms_v5', nbytes=28 * n * K, kernels=2)
     self.launches_per_forward = sum(i['kernels'] for i in self.op_info)
+
+  def _build_segmentation(self, w):
+    """SegmentationHead (tf2/efficientdet_keras.py:694-706) after the last BiFPN cell, as one
+    graph branch: every stage is one edet_conv2d_transpose with BN folded into its weights, whose
+    two K sources are the previous stage's output and the BiFPN level of the reference's concat
+    (the concat is never written).  self.seg_out: fp16 [N, 2H_min, 2W_min, round8(C)]."""
+    a, n = self.arch, self.n
+    self.seg_out = None
+    if not a.seg_stages:
+      return
+    f16, f32 = torch.float16, torch.float32
+    F = a.fpn_filters
+    self._branch = 'segmentation_head'
+    x, skip = self.fpn_feats[a.max_level], None
+    for st in a.seg_stages:
+      kernel = np.asarray(w[st.kernel_scope + '/kernel'], np.float64)   # [3, 3, out, in]
+      if st.bn_scope:
+        scale, bias = _bn_fold(w, st.bn_scope, a.bn_eps)
+        act = self.act
+      else:
+        scale, bias = None, np.asarray(w[st.kernel_scope + '/bias'], np.float64)
+        act = utils.ACT_NONE
+      cout = st.out_channels
+      wt = self._dev(ops.conv_transpose_weights(kernel, F, scale), f16)
+      b = self._dev(bias, f32)
+      oh, ow = st.out_hw
+      y = self._buf(st.kernel_scope, (n, oh, ow, _round_up(cout, 8)))
+      ih, iw = st.in_hw
+      self._add(st.kernel_scope,
+                lambda x=x, skip=skip, wt=wt, b=b, y=y, act=act, cout=cout:
+                ops.conv2d_transpose(x, wt, b, y, act, cout, a1=skip),
+                kind='conv_transpose_tc',
+                nbytes=2 * n * (ih * iw * st.in_channels + oh * ow * y.shape[-1]) + 2 * wt.numel(),
+                flops=18 * n * ih * iw * st.in_channels * cout)
+      x, skip = y, (self.fpn_feats[st.skip_level] if st.skip_level is not None else None)
+    self.seg_out = x
+    self._branch = None
 
   # ---- execution ------------------------------------------------------------------------------
   def _run_ops(self, upto=None, parallel_branches=True, start=0, priority=0):
@@ -650,6 +692,9 @@ class Engine(object):
       `self.detections` from the current stream.
     """
     net_upto = self.num_network_ops
+    if postprocess and not self.arch.has_detection:
+      raise ValueError('post-processing needs the object_detection head; config.heads = %s'
+                       % (self.arch.heads,))
     if not postprocess:
       self.flush()
       self._logits_current = True
@@ -808,6 +853,14 @@ class Engine(object):
     return ({l: t[..., :A * C] for l, t in self.cls_out.items()},
             {l: t[..., :A * 4] for l, t in self.box_out.items()})
 
+  @property
+  def seg_logits(self):
+    """fp16 [N, 2H_min, 2W_min, seg_num_classes] view of the segmentation head's output (written
+    by every forward / run; None without the head)."""
+    if self.seg_out is None:
+      return None
+    return self.seg_out[..., :self.arch.config.seg_num_classes]
+
   def detect(self, images=None, image_scales=None):
     """Network + post-process: float32 [N, max_output_size, 7] device tensor."""
     with torch.cuda.device(self.device):
@@ -824,6 +877,9 @@ class Engine(object):
     {'boxes' [N,K,4], 'scores' [N,K], 'classes' [N,K]} (for the per-class NMS path,
     automl_b200/postprocess.py).  After forward() it is computed here from the head outputs;
     after run(postprocess=True) / detect() it is what that step already produced."""
+    if not self.arch.has_detection:
+      raise ValueError('pre-NMS needs the object_detection head; config.heads = %s'
+                       % (self.arch.heads,))
     with torch.cuda.device(self.device):
       self.flush()
       main = torch.cuda.current_stream(self.device)

@@ -6,6 +6,7 @@ implementation behind any of them.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from automl_b200 import _lib
@@ -98,6 +99,58 @@ def conv2d(x, wt, bias, out, act, ksize, stride, residual=None):
   _lib.call('edet_conv2d', _ptr(x, torch.float16), _ptr(wt, torch.float16),
             _ptr(bias, torch.float32), _ptr(residual, torch.float16), _ptr(out, torch.float16),
             n, h, w, cin, cout, ksize, stride, act, _stream())
+
+
+def conv_transpose_weights(kernel, c0, scale=None):
+  """Packs a Keras Conv2DTranspose kernel [3, 3, cout, cin] (float, cin = c0 + c1) into the
+  float64 [4 taps][4 * round8(cout)][round8(c0) + round8(c1)] sub-pixel layout of
+  edet_conv2d_transpose: row (py*2+px)*C8 + co of tap ty*2+tx is kernel[ky, kx, co] for output
+  phase (py, px), ky = 1 if py else (2 if ty == 0 else 0) (kx alike), zero for ty < py or tx < px.
+  Input channels [0, c0) go to columns [0, c0), the rest to columns round8(c0)...  `scale`
+  [cout] (the folded BN scale) multiplies each output channel."""
+  kernel = np.asarray(kernel, np.float64)
+  kh, kw, cout, cin = kernel.shape
+  assert (kh, kw) == (3, 3) and 0 < c0 <= cin
+  if scale is not None:
+    kernel = kernel * np.asarray(scale, np.float64)[:, None]
+  c8, c1 = _round8(cout), cin - c0
+  off1 = _round8(c0)
+  out = np.zeros((4, 4 * c8, off1 + _round8(c1)), np.float64)
+  for py in range(2):
+    for px in range(2):
+      rows = slice((py * 2 + px) * c8, (py * 2 + px) * c8 + cout)
+      for ty in range(py, 2):
+        for tx in range(px, 2):
+          ky = 1 if py else (2 if ty == 0 else 0)
+          kx = 1 if px else (2 if tx == 0 else 0)
+          out[ty * 2 + tx, rows, :c0] = kernel[ky, kx, :, :c0]
+          out[ty * 2 + tx, rows, off1:off1 + c1] = kernel[ky, kx, :, c0:]
+  return out
+
+
+def conv2d_transpose(a0, wt, bias, out, act, cout, a1=None, c0=None, c1=None):
+  """Conv2DTranspose 3x3 stride 2 'SAME' + bias + act on the tensor cores: a0 fp16 [N,H,W,lda0]
+  (channels [0, c0), c0 defaults to lda0), a1 None or fp16 [N,H,W,lda1] (channels [0, c1)) read as
+  the K channels after a0's, wt fp16 from conv_transpose_weights, bias fp32 [cout], out fp16
+  [N,2H,2W,ldo] with ldo >= round8(cout)."""
+  n, h, w, lda0 = a0.shape
+  c0 = lda0 if c0 is None else c0
+  lda1 = 0
+  if a1 is not None:
+    assert tuple(a1.shape[:3]) == (n, h, w)
+    lda1 = a1.shape[-1]
+    c1 = lda1 if c1 is None else c1
+  else:
+    c1 = 0
+  if tuple(out.shape[:3]) != (n, 2 * h, 2 * w):
+    raise ValueError('conv2d_transpose: out must be [%d, %d, %d, ldo], got %s'
+                     % (n, 2 * h, 2 * w, tuple(out.shape)))
+  if tuple(wt.shape) != (4, 4 * _round8(cout), _round8(c0) + _round8(c1)):
+    raise ValueError('conv2d_transpose: wt shape %s does not match cout %d, c0 %d, c1 %d'
+                     % (tuple(wt.shape), cout, c0, c1))
+  _lib.call('edet_conv2d_transpose', _ptr(a0, torch.float16), c0, lda0, _ptr(a1, torch.float16),
+            c1, lda1, _ptr(wt, torch.float16), _ptr(bias, torch.float32), act,
+            _ptr(out, torch.float16), out.shape[-1], n, h, w, cout, _stream())
 
 
 def mbconv_expand_dw(x, we, bias_e, wd, bias_d, out, act, k, stride, se_sum=None):

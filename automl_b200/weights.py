@@ -93,9 +93,9 @@ def variable_specs(arch):
       s[node.op_scope + '/conv/bias'] = VarSpec((f,), 'bias', True)
       _bn(s, node.op_scope + '/bn', f)
 
-  for net, pred_c, pred_kind in (('class', arch.num_classes * arch.num_anchors,
-                                  'class_bias'),
-                                 ('box', 4 * arch.num_anchors, 'bias')):
+  dets = ((('class', arch.num_classes * arch.num_anchors, 'class_bias'),
+           ('box', 4 * arch.num_anchors, 'bias')) if arch.has_detection else ())
+  for net, pred_c, pred_kind in dets:
     scope = '%s_net' % net
     for i in range(arch.head_repeats):
       s['%s/%s-%d/depthwise_kernel' % (scope, net, i)] = VarSpec(
@@ -110,6 +110,16 @@ def variable_specs(arch):
     s['%s/%s-predict/pointwise_kernel' % (scope, net)] = VarSpec(
         (1, 1, f, pred_c), 'sep_pw', True)
     s['%s/%s-predict/bias' % (scope, net)] = VarSpec((pred_c,), pred_kind, True)
+
+  # segmentation head (tf2/efficientdet_keras.py:676-692), only when configured; the names are
+  # Keras' default layer names (arch._seg_stages), not checkable offline
+  for st in arch.seg_stages:
+    s[st.kernel_scope + '/kernel'] = VarSpec((3, 3, st.out_channels, st.in_channels),
+                                             'conv_transpose', True)
+    if st.bn_scope:
+      _bn(s, st.bn_scope, st.out_channels)
+    else:
+      s[st.kernel_scope + '/bias'] = VarSpec((st.out_channels,), 'bias', True)
   return s
 
 
@@ -139,6 +149,12 @@ def synthetic_weights(arch, seed=0):
         # fan_in scaling keeps 200 stacked layers O(1) with swish in between.
         std = math.sqrt(2.0 / (kh * kw * cin))
       w = rng.normal(0.0, std, size=shape)
+    elif kind == 'conv_transpose':
+      # Keras' default glorot_uniform on the (kh, kw, out, in) kernel: fan_in = kh*kw*out,
+      # fan_out = kh*kw*in (Conv2DTranspose keeps the reference's default initialiser)
+      kh, kw, cout, cin = shape
+      limit = math.sqrt(6.0 / (kh * kw * (cout + cin)))
+      w = rng.uniform(-limit, limit, size=shape)
     elif kind == 'gamma':
       w = rng.uniform(0.8, 1.2, size=shape)
     elif kind == 'beta':

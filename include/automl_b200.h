@@ -106,6 +106,25 @@ int edet_conv2d(const edet_half* in, const edet_half* wt, const float* bias,
                 const edet_half* residual, edet_half* out, int n, int h, int w, int cin, int cout,
                 int ksize, int stride, int act, edet_stream_t stream);
 
+/* Conv2DTranspose 3x3 stride 2 'SAME' (TF conv2d_transpose: the adjoint of the k3 s2 'SAME'
+ * conv2d, output 2h x 2w) + bias (BN folded) + act, with the input channels read from one or two
+ * sources (the second follows the first in K: a channel concat that is never written), as a
+ * sub-pixel implicit GEMM on the tensor cores (wgmma).  Replaces the Conv2DTranspose + BN + act +
+ * concat of each upsampling stage and the final Conv2DTranspose of SegmentationHead,
+ * tf2/efficientdet_keras.py:676-706.
+ *   a0  half [n, h, w, lda0], channels [0, c0)        a1  half [n, h, w, lda1], channels [0, c1),
+ *                                                          or NULL (c1, lda1 ignored)
+ *   wt  half [4][4 * C8][round8(c0) + round8(c1)], C8 = round8(cout): row (py*2+px)*C8 + co of tap
+ *       ty*2+tx is Keras kernel[ky, kx, co, :] of output phase (py, px) (ky = 1 if py else
+ *       (ty ? 0 : 2), kx alike; zero for the tap-phase pairs with ty < py or tx < px), columns
+ *       [0, c0) for a0 and [round8(c0), round8(c0) + c1) for a1, zero elsewhere; BN scale folded
+ *   bias float32 [cout]                  out half [n, 2h, 2w, ldo]: channels [0, cout) written,
+ *                                        [cout, C8) set to zero, [C8, ldo) untouched
+ *   lda0, lda1, ldo multiples of 8, ldo >= C8; act in {NONE, SWISH, RELU6}. */
+int edet_conv2d_transpose(const edet_half* a0, int c0, int lda0, const edet_half* a1, int c1,
+                          int lda1, const edet_half* wt, const float* bias, int act, edet_half* out,
+                          int ldo, int n, int h, int w, int cout, edet_stream_t stream);
+
 /* Fused front half of an MBConv block: expand 1x1 + BN + act  ->  depthwise kxk 'SAME' + BN +
  * act (+ SE squeeze), the expanded [N,H,W,cmid] tensor never leaves the SM (wgmma accumulators
  * in registers -> fp16 tile in shared memory -> depthwise).  Same results as edet_pointwise_conv
