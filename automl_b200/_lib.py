@@ -56,6 +56,8 @@ SIGNATURES = {
                            c_int, c_int, c_void_p]),
     'edet_fuse_dw': (c_int, [ctypes.POINTER(FuseInput), c_int, c_void_p, c_void_p, c_int, c_int,
                              c_int, c_int, c_int, c_void_p]),
+    'edet_fuse_dw_channel': (c_int, [ctypes.POINTER(FuseInput), c_int, c_void_p, c_void_p, c_void_p,
+                                     c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'edet_sepconv': (c_int, [ctypes.POINTER(FuseInput), c_int, c_int, c_void_p, c_void_p, c_void_p,
                              c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'edet_max_pool': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,

@@ -106,14 +106,17 @@ class DetArch(object):
       raise ValueError('bad data_format %r' % (p.data_format,))
     if not p.separable_conv:
       raise NotImplementedError('separable_conv=False is not on the H100 path')
-    if p.conv_bn_act_pattern or p.conv_after_downsample:
-      raise NotImplementedError(
-          'conv_bn_act_pattern / conv_after_downsample variants (SURVEY 8f.4)')
     if p.backbone_config is not None:
       raise NotImplementedError('custom backbone_config')
     self.config = p
     self._resolve_heads(p)
     self.act_type = p.act_type
+    # node op: fuse -> sepconv without bias -> BN -> act instead of fuse -> act -> sepconv + bias
+    # -> BN (efficientdet_arch.py:508-533)
+    self.conv_bn_act_pattern = bool(p.conv_bn_act_pattern)
+    # a shrinking resample with a channel change max-pools first and applies its 1x1 conv + BN
+    # at the pooled size (efficientdet_arch.py:100-115)
+    self.conv_after_downsample = bool(p.conv_after_downsample)
     self.image_hw = utils.parse_image_size(p.image_size)
     self.min_level, self.max_level = p.min_level, p.max_level
     self.num_levels = p.max_level - p.min_level + 1
@@ -248,6 +251,10 @@ class DetArch(object):
           'which is a width concat there, not a channel concat')
 
   # -- convenience ---------------------------------------------------------------
+  def conv_after_pool(self, r):
+    """True when resample `r` applies its 1x1 conv after the max-pool, at r.out_hw."""
+    return self.conv_after_downsample and r.has_conv and r.mode == 'down'
+
   @property
   def levels(self):
     return list(range(self.min_level, self.max_level + 1))

@@ -16,19 +16,23 @@ constexpr int kFuseCB = 32;                // channels per CTA
 // phase-2 loads (4 channel groups x 2 columns) hit 8 distinct bank groups.
 constexpr int kFusePitch = kFuseCB + 4;
 
-// SIG: compile-time input signature (fuse_common.cuh: kSigGeneric or one of the three shapes a
-// BiFPN cell has).  With the modes known at compile time the loads of ALL inputs of an item
+// SIG: compile-time input signature (fuse_common.cuh: kSigGeneric or one of the node shapes of a
+// BiFPN / QuFPN cell).  With the modes known at compile time the loads of ALL inputs of an item
 // are issued before any of them is consumed (the generic loop serialises one global round trip
 // per input: the kernel is latency bound, ncu long-scoreboard 5.0 issue-slots per instruction).
-template <int ACT, int SIG>
-__global__ void __launch_bounds__(kFuseThreads)
-fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __restrict__ out,
-               int h, int wd, int c, int chunks) {
+// CW: per-channel fusion weights fuse_w [n_inputs][c] (channel_attn / channel_fastattn) instead of
+// the scalar FuseIn::weight; same ffma2_rn chain, so weights equal across channels give the bits
+// of the scalar form.
+template <int ACT, int SIG, bool CW>
+__device__ __forceinline__ void fuse_dw_body(const FuseParams& p, const float* __restrict__ dw_w,
+                                             __half* __restrict__ out, int h, int wd, int c,
+                                             int chunks, const float* __restrict__ fuse_w) {
   pdl_launch_dependents();
   constexpr int HT = kFuseTH + 2, WT = kFuseTW + 2, G = kFuseCB / 8;
   static_assert(G == 4 && kFuseTH * kFuseTW * G == 2 * kFuseThreads, "phase-2 mapping");
   __shared__ __align__(16) float fused[HT * WT * kFusePitch];
   __shared__ __align__(16) float wsm[9 * kFuseCB];
+  __shared__ __align__(16) float fwsm[CW ? kFuseMaxIn * kFuseCB : 1];
   const int n = blockIdx.z / chunks;
   const int c0 = (blockIdx.z % chunks) * kFuseCB;
   const int y0 = blockIdx.y * kFuseTH, x0 = blockIdx.x * kFuseTW;
@@ -38,7 +42,19 @@ fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __res
     const int tap = i / kFuseCB, ch = i % kFuseCB;
     wsm[i] = (c0 + ch < c) ? __ldg(dw_w + static_cast<size_t>(tap) * c + c0 + ch) : 0.f;
   }
+  if constexpr (CW) {   // per-channel fusion weights of this chunk (constants, like the taps)
+    for (int i = threadIdx.x; i < p.n_inputs * kFuseCB; i += kFuseThreads) {
+      const int in = i / kFuseCB, ch = i % kFuseCB;
+      fwsm[i] = (c0 + ch < c) ? __ldg(fuse_w + static_cast<size_t>(in) * c + c0 + ch) : 0.f;
+    }
+    __syncthreads();    // read in phase 1 by other threads (the taps only after phase 1's barrier)
+  }
   pdl_wait_prior();
+  // weights of channel pair e of group g of input i
+  auto wpair = [&](int i, int g, int e) {
+    if constexpr (CW) return reinterpret_cast<const float2*>(fwsm + i * kFuseCB + g * 8)[e];
+    else return make_float2(p.in[i].weight, p.in[i].weight);
+  };
 
   // ---- phase 1: fused + activated map for the tile and its 1-pixel halo -------------------
   for (int item = threadIdx.x; item < HT * WT * G; item += kFuseThreads) {
@@ -56,9 +72,8 @@ fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __res
           const __half* base = fi.ptr + static_cast<size_t>(n) * fi.h * fi.w * c;
           float v[8];
           resample8(fi, base, c, y, x, ch, v);
-          const float2 w2 = make_float2(fi.weight, fi.weight);
 #pragma unroll
-          for (int e = 0; e < 4; ++e) acc[e] = ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), w2, acc[e]);
+          for (int e = 0; e < 4; ++e) acc[e] = ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), wpair(i, g, e), acc[e]);
         }
       } else {
         // all raw loads first (same values, same accumulation order as the generic loop)
@@ -69,19 +84,18 @@ fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __res
         taps0 = resample_raw<sig_mode(SIG, 0)>(p.in[0], img(0), c, y, x, ch, raw0);
         taps1 = resample_raw<sig_mode(SIG, 1)>(p.in[1], img(1), c, y, x, ch, raw1);
         if (NI == 3) taps2 = resample_raw<sig_mode(SIG, 2)>(p.in[2], img(2), c, y, x, ch, raw2);
-        auto accumulate = [&](const float* v, float weight) {
-          const float2 w2 = make_float2(weight, weight);
+        auto accumulate = [&](const float* v, int i) {
 #pragma unroll
-          for (int e = 0; e < 4; ++e) acc[e] = ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), w2, acc[e]);
+          for (int e = 0; e < 4; ++e) acc[e] = ffma2_rn(make_float2(v[2 * e], v[2 * e + 1]), wpair(i, g, e), acc[e]);
         };
         float v[8];
         resample_reduce<sig_mode(SIG, 0)>(raw0, taps0, v);
-        accumulate(v, p.in[0].weight);
+        accumulate(v, 0);
         resample_reduce<sig_mode(SIG, 1)>(raw1, taps1, v);
-        accumulate(v, p.in[1].weight);
+        accumulate(v, 1);
         if (NI == 3) {
           resample_reduce<sig_mode(SIG, 2)>(raw2, taps2, v);
-          accumulate(v, p.in[2].weight);
+          accumulate(v, 2);
         }
       }
       apply_act4<ACT>(acc[0], acc[1]);
@@ -140,6 +154,23 @@ fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __res
   }
 }
 
+template <int ACT, int SIG>
+__global__ void __launch_bounds__(kFuseThreads)
+fuse_dw_kernel(const FuseParams p, const float* __restrict__ dw_w, __half* __restrict__ out,
+               int h, int wd, int c, int chunks) {
+  fuse_dw_body<ACT, SIG, false>(p, dw_w, out, h, wd, c, chunks, nullptr);
+}
+
+// The per-channel weights keep up to 24 more values live in phase 1; left to itself ptxas trades
+// them for spills; the register budget of two CTAs per SM (up to 128 per thread) avoids that.
+template <int ACT, int SIG>
+__global__ void __launch_bounds__(kFuseThreads, 2)
+fuse_dw_channel_kernel(const FuseParams p, const float* __restrict__ fuse_w,
+                       const float* __restrict__ dw_w, __half* __restrict__ out, int h, int wd,
+                       int c, int chunks) {
+  fuse_dw_body<ACT, SIG, true>(p, dw_w, out, h, wd, c, chunks, fuse_w);
+}
+
 __global__ void __launch_bounds__(256)
 max_pool_kernel(const __half* __restrict__ in, __half* __restrict__ out, int h, int wd, int c,
                 int ho, int wo, int pool_h, int pool_w, int stride_h, int stride_w, int pad_t,
@@ -177,14 +208,18 @@ max_pool_kernel(const __half* __restrict__ in, __half* __restrict__ out, int h, 
 
 }  // namespace edet
 
-extern "C" int edet_fuse_dw(const edet_fuse_input* h_inputs, int n_inputs, const float* dw_w,
-                            edet_half* out, int n, int h, int wd, int c, int act,
-                            edet_stream_t stream) {
-  using namespace edet;
-  EDET_CHECK_ARG(dw_w && out, "fuse_dw: null pointer");
-  EDET_CHECK_ARG(n > 0 && h > 0 && wd > 0 && c > 0 && c % 8 == 0, "fuse_dw: bad shape");
+namespace edet {
+namespace {
+
+template <bool CW>
+int launch_fuse_dw(const edet_fuse_input* h_inputs, int n_inputs, const float* fuse_w,
+                   const float* dw_w, edet_half* out, int n, int h, int wd, int c, int act,
+                   edet_stream_t stream, const char* who) {
+  EDET_CHECK_ARG(dw_w && out, "%s: null pointer", who);
+  EDET_CHECK_ARG(!CW || fuse_w, "%s: null fusion weights", who);
+  EDET_CHECK_ARG(n > 0 && h > 0 && wd > 0 && c > 0 && c % 8 == 0, "%s: bad shape", who);
   FuseParams p;
-  if (int rc = fill_fuse_params(h_inputs, n_inputs, h, wd, "fuse_dw", &p)) return rc;
+  if (int rc = fill_fuse_params(h_inputs, n_inputs, h, wd, who, &p)) return rc;
   const int chunks = ceil_div(c, kFuseCB);
   dim3 grid(ceil_div(wd, kFuseTW), ceil_div(h, kFuseTH), n * chunks);
   const float* hw = dw_w;
@@ -192,12 +227,17 @@ extern "C" int edet_fuse_dw(const edet_fuse_input* h_inputs, int n_inputs, const
   cudaStream_t s = as_stream(stream);
   cudaError_t err = cudaSuccess;
   const int sig = fuse_signature(p);
-#define EDET_FUSE_DW(ACT)                                                                          \
-  switch (sig) {                                                                                   \
-    case kSigSameUp: err = launch_pdl(fuse_dw_kernel<ACT, kSigSameUp>, grid, dim3(kFuseThreads), 0, s, p, hw, ho, h, wd, c, chunks); break; \
-    case kSigSameSameDown: err = launch_pdl(fuse_dw_kernel<ACT, kSigSameSameDown>, grid, dim3(kFuseThreads), 0, s, p, hw, ho, h, wd, c, chunks); break; \
-    case kSigSameDown: err = launch_pdl(fuse_dw_kernel<ACT, kSigSameDown>, grid, dim3(kFuseThreads), 0, s, p, hw, ho, h, wd, c, chunks); break; \
-    default: err = launch_pdl(fuse_dw_kernel<ACT, kSigGeneric>, grid, dim3(kFuseThreads), 0, s, p, hw, ho, h, wd, c, chunks); break; \
+#define EDET_FUSE_DW_SIG(ACT, SIG)                                                                  \
+  err = CW ? launch_pdl(fuse_dw_channel_kernel<ACT, SIG>, grid, dim3(kFuseThreads), 0, s, p, fuse_w, hw, ho, h, wd, c, chunks) \
+           : launch_pdl(fuse_dw_kernel<ACT, SIG>, grid, dim3(kFuseThreads), 0, s, p, hw, ho, h, wd, c, chunks)
+#define EDET_FUSE_DW(ACT)                                                                      \
+  switch (sig) {                                                                               \
+    case kSigSameUp: EDET_FUSE_DW_SIG(ACT, kSigSameUp); break;                                 \
+    case kSigSameSameDown: EDET_FUSE_DW_SIG(ACT, kSigSameSameDown); break;                     \
+    case kSigSameDown: EDET_FUSE_DW_SIG(ACT, kSigSameDown); break;                             \
+    case kSigSameSame: EDET_FUSE_DW_SIG(ACT, kSigSameSame); break;                             \
+    case kSigSameSameUp: EDET_FUSE_DW_SIG(ACT, kSigSameSameUp); break;                         \
+    default: EDET_FUSE_DW_SIG(ACT, kSigGeneric); break;                                        \
   }
   switch (act) {
     case EDET_ACT_SWISH: EDET_FUSE_DW(EDET_ACT_SWISH); break;
@@ -206,12 +246,30 @@ extern "C" int edet_fuse_dw(const edet_fuse_input* h_inputs, int n_inputs, const
     case EDET_ACT_HSWISH: EDET_FUSE_DW(EDET_ACT_HSWISH); break;
     case EDET_ACT_NONE: EDET_FUSE_DW(EDET_ACT_NONE); break;
     default:
-      set_error("fuse_dw: bad activation %d", act);
+      set_error("%s: bad activation %d", who, act);
       return EDET_ERR_INVALID;
   }
 #undef EDET_FUSE_DW
+#undef EDET_FUSE_DW_SIG
   EDET_CHECK_CUDA(err);
   return EDET_OK;
+}
+
+}  // namespace
+}  // namespace edet
+
+extern "C" int edet_fuse_dw(const edet_fuse_input* h_inputs, int n_inputs, const float* dw_w,
+                            edet_half* out, int n, int h, int wd, int c, int act,
+                            edet_stream_t stream) {
+  return edet::launch_fuse_dw<false>(h_inputs, n_inputs, nullptr, dw_w, out, n, h, wd, c, act,
+                                     stream, "fuse_dw");
+}
+
+extern "C" int edet_fuse_dw_channel(const edet_fuse_input* h_inputs, int n_inputs,
+                                    const float* fuse_w, const float* dw_w, edet_half* out, int n,
+                                    int h, int wd, int c, int act, edet_stream_t stream) {
+  return edet::launch_fuse_dw<true>(h_inputs, n_inputs, fuse_w, dw_w, out, n, h, wd, c, act,
+                                    stream, "fuse_dw_channel");
 }
 
 extern "C" int edet_max_pool(const edet_half* in, edet_half* out, int n, int h, int wd, int c,

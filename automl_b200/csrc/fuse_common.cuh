@@ -61,11 +61,18 @@ __device__ __forceinline__ void resample8(const FuseIn& fi, const __half* base, 
 // A BiFPN cell (tf2/fpn_configs.py:24-72) only has three node shapes: top-down nodes read
 // [same level, upsampled coarser level]; bottom-up nodes read [same level input, same level
 // top-down output, pooled finer level]; the topmost bottom-up node reads [same level, pooled].
-constexpr int kSigGeneric = 0, kSigSameUp = 1, kSigSameSameDown = 2, kSigSameDown = 3;
-__host__ __device__ constexpr int sig_inputs(int sig) { return sig == kSigSameSameDown ? 3 : 2; }
+// A QuFPN cell (:75-163) adds two: the quad-add nodes read [same, same], the nodes of its
+// second top-down path read [same level input, same level path-3 output, upsampled coarser level].
+constexpr int kSigGeneric = 0, kSigSameUp = 1, kSigSameSameDown = 2, kSigSameDown = 3,
+              kSigSameSame = 4, kSigSameSameUp = 5;
+__host__ __device__ constexpr int sig_inputs(int sig) {
+  return (sig == kSigSameSameDown || sig == kSigSameSameUp) ? 3 : 2;
+}
 __host__ __device__ constexpr int sig_mode(int sig, int i) {
   return sig == kSigSameUp         ? (i == 0 ? EDET_RS_SAME : EDET_RS_UP)
          : sig == kSigSameSameDown ? (i < 2 ? EDET_RS_SAME : EDET_RS_DOWN)
+         : sig == kSigSameSame     ? EDET_RS_SAME
+         : sig == kSigSameSameUp   ? (i < 2 ? EDET_RS_SAME : EDET_RS_UP)
                                    : (i == 0 ? EDET_RS_SAME : EDET_RS_DOWN);
 }
 inline int fuse_signature(const FuseParams& p) {
@@ -76,6 +83,9 @@ inline int fuse_signature(const FuseParams& p) {
   if (p.n_inputs == 3 && is(0, EDET_RS_SAME) && is(1, EDET_RS_SAME) && is(2, EDET_RS_DOWN) && pool33(2))
     return kSigSameSameDown;
   if (p.n_inputs == 2 && is(0, EDET_RS_SAME) && is(1, EDET_RS_DOWN) && pool33(1)) return kSigSameDown;
+  if (p.n_inputs == 2 && is(0, EDET_RS_SAME) && is(1, EDET_RS_SAME)) return kSigSameSame;
+  if (p.n_inputs == 3 && is(0, EDET_RS_SAME) && is(1, EDET_RS_SAME) && is(2, EDET_RS_UP))
+    return kSigSameSameUp;
   return kSigGeneric;
 }
 

@@ -287,8 +287,9 @@ class Engine(object):
     check_c(F, 'fpn_num_filters')
 
     def resample_conv(r, src):
-      """1x1 conv(+bias)+BN of a resample op at the SOURCE resolution (conv_after_downsample
-      is False for every registered model)."""
+      """1x1 conv(+bias)+BN of a resample op at the SOURCE resolution, or, when
+      conv_after_downsample moves it behind the max-pool (a.conv_after_pool), max-pool then
+      conv at the TARGET resolution: the result then enters the node as a 'same' input."""
       kw = np.asarray(w[r.scope + '/conv2d/kernel'], np.float64)[0, 0]  # [Cin,F]
       cb = np.asarray(w[r.scope + '/conv2d/bias'], np.float64)
       if a.config.apply_bn_for_resampling:
@@ -297,9 +298,19 @@ class Engine(object):
         s, sh = np.ones(F), np.zeros(F)
       wt = self._dev((kw * s).T, f16)
       bias = self._dev(cb * s + sh, f32)
-      out = self._buf(r.scope + '/conv', (n, r.in_hw[0], r.in_hw[1], F))
       # a detached branch ('~' prefix): only the op that consumes `out` joins it
-      self._pw(r.scope + '/conv', src, wt, bias, out, utils.ACT_NONE, branch='~' + r.scope)
+      branch = '~' + r.scope
+      hh, ww = r.in_hw
+      if a.conv_after_pool(r):
+        check_c(r.in_channels, r.scope)
+        hh, ww = r.out_hw
+        pooled = self._buf(r.scope + '/pool', (n, hh, ww, r.in_channels))
+        self._add(r.scope + '/pool',
+                  lambda src=src, pooled=pooled, r=r: ops.max_pool(src, pooled, r.pool[:2], r.pool[2:]),
+                  kind='max_pool', nbytes=2 * (src.numel() + pooled.numel()), branch=branch)
+        src = pooled
+      out = self._buf(r.scope + '/conv', (n, hh, ww, F))
+      self._pw(r.scope + '/conv', src, wt, bias, out, utils.ACT_NONE, branch=branch)
       return out
 
     pyramid = []
@@ -318,15 +329,18 @@ class Engine(object):
         for r in node.inputs:
           if r.has_conv and r.src < len(pyramid):
             hoisted[r.scope] = resample_conv(r, pyramid[r.src])
+    level_needs = {}   # pyramid index -> detached branch that writes the level
     for r in a.extra_levels:
       src = pyramid[r.src]
-      needs = []
+      needs = list(level_needs.get(r.src, []))
       if r.has_conv:
         src = hoisted[r.scope]
-        needs = ['~' + r.scope]
-      if r.mode == 'same':
+        needs.append('~' + r.scope)
+      if r.mode == 'same' or a.conv_after_pool(r):
         # 1x1 maps cannot shrink further: the reference only applies the (optional) 1x1 conv
-        # (efficientdet_arch.py:116-117), so the level aliases its source.
+        # (efficientdet_arch.py:116-117), so the level aliases its source; with
+        # conv_after_downsample the hoisted op already pooled before its conv.
+        level_needs[len(pyramid)] = needs
         pyramid.append(src)
         continue
       if r.mode != 'down':
@@ -342,11 +356,15 @@ class Engine(object):
     # feature networks keep the fuse_dw + pointwise pair
     fuse_sep = (self.fuse_sepconv and F <= ops.SEPCONV_MAX_C and
                 act in (utils.ACT_SWISH, utils.ACT_RELU6))
+    # conv_bn_act_pattern: the activation moves from the fusion to the pointwise epilogue
+    node_pre_act, node_post_act = (utils.ACT_NONE, act) if a.conv_bn_act_pattern else (act, utils.ACT_NONE)
     for ci, cell in enumerate(a.cells):
       cell_feats = list(pyramid)
       for node in cell['nodes']:
         specs = []
-        # fusion weights (efficientdet_arch.py:439-447), float32 like the reference
+        cw = None     # per-channel weights [inputs, F] of the channel_* methods
+        wsm = lambda i, node=node: w['%s/WSM%s' % (node.scope, '' if i == 0 else '_%d' % i)]
+        # fusion weights (efficientdet_arch.py:439-468), float32 like the reference
         if a.fpn_weight_method == 'fastattn':
           ew = [np.maximum(np.float32(w['%s/WSM%s' % (node.scope, '' if i == 0 else '_%d' % i)]),
                            np.float32(0)) for i in range(len(node.inputs))]
@@ -359,23 +377,43 @@ class Engine(object):
           fw = list(ex / ex.sum())
         elif a.fpn_weight_method == 'sum':
           fw = [1.0] * len(node.inputs)
+        elif a.fpn_weight_method == 'channel_fastattn':
+          # per channel: relu(w_i) / (sum_j relu(w_j) + 1e-4), summed in input order like add_n
+          ew = [np.maximum(np.asarray(wsm(i), np.float32), np.float32(0)) for i in range(len(node.inputs))]
+          tot = ew[0]
+          for e in ew[1:]:
+            tot = tot + e
+          tot = tot + np.float32(0.0001)
+          cw = np.stack([e / tot for e in ew])
+        elif a.fpn_weight_method == 'channel_attn':
+          ev = np.stack([np.asarray(wsm(i), np.float32) for i in range(len(node.inputs))])
+          ex = np.exp(ev - ev.max(axis=0))       # softmax over the inputs, per channel
+          cw = ex / ex.sum(axis=0)
         else:
           raise NotImplementedError('fpn_weight_method %s' % a.fpn_weight_method)
+        if cw is not None:
+          fw = [1.0] * len(node.inputs)          # ignored by the per-channel entry point
+          cw = self._dev(cw.astype(np.float32), f32)
         needs = []
         for r, wgt in zip(node.inputs, fw):
           src = cell_feats[r.src]
+          mode, pool = r.mode, r.pool
           if r.has_conv:
             if r.scope in hoisted:
               src = hoisted[r.scope]
             else:
               src = resample_conv(r, src)
             needs.append('~' + r.scope)
-          specs.append((src, mode_code[r.mode], r.pool, float(wgt)))
+            if a.conv_after_pool(r):
+              mode, pool = 'same', None
+          elif ci == 0:
+            needs.extend(level_needs.get(r.src, []))
+          specs.append((src, mode_code[mode], pool, float(wgt)))
         op = node.op_scope
         dw_w = self._dev(np.asarray(w[op + '/conv/depthwise_kernel'], np.float64)[..., 0].reshape(9, F), f32)
         s, sh = _bn_fold(w, op + '/bn', eps)
         kp = np.asarray(w[op + '/conv/pointwise_kernel'], np.float64)[0, 0]
-        cb = np.asarray(w[op + '/conv/bias'], np.float64)
+        cb = 0.0 if a.conv_bn_act_pattern else np.asarray(w[op + '/conv/bias'], np.float64)
         pw_wt = self._dev((kp * s).T, f16)
         pw_b = self._dev(cb * s + sh, f32)
         hh, ww = node.hw
@@ -383,10 +421,12 @@ class Engine(object):
         in_bytes = 2 * sum(sp[0].numel() for sp in specs)
         tmp = self._buf(node.scope + '/fused_dw', (n, hh, ww, F))
         self._add(node.scope + '/fuse_dw',
-                  lambda specs=specs, dw_w=dw_w, tmp=tmp: ops.fuse_dw(specs, dw_w, tmp, act),
-                  kind='bifpn_fuse_dw', nbytes=in_bytes + 2 * tmp.numel() + 18 * F,
+                  lambda specs=specs, dw_w=dw_w, tmp=tmp, cw=cw:
+                  ops.fuse_dw(specs, dw_w, tmp, node_pre_act, channel_weights=cw),
+                  kind='bifpn_fuse_dw',
+                  nbytes=in_bytes + 2 * tmp.numel() + 18 * F + (cw.numel() * 4 if cw is not None else 0),
                   flops=2 * 9 * tmp.numel(), needs=needs)
-        self._pw(node.scope + '/pw', tmp, pw_wt, pw_b, out, utils.ACT_NONE)
+        self._pw(node.scope + '/pw', tmp, pw_wt, pw_b, out, node_post_act)
         cell_feats.append(out)
       pyramid = [cell_feats[cell['out_index'][l]] for l in a.levels]
       if ci == 0:

@@ -195,13 +195,22 @@ def make_fuse_inputs(specs):
   return arr
 
 
-def fuse_dw(specs, dw_w, out, act):
+def fuse_dw(specs, dw_w, out, act, channel_weights=None):
+  """channel_weights: None (each spec's scalar weight) or fp32 [len(specs), C], the normalised
+  per-channel fusion weights of the channel_* methods (the specs' weights are then ignored)."""
   n, h, wd, c = out.shape
   for t, _, _, _ in specs:
     _ptr(t, torch.float16)
   arr = make_fuse_inputs(specs)
-  _lib.call('edet_fuse_dw', arr, len(specs), _ptr(dw_w, torch.float32),
-            _ptr(out, torch.float16), n, h, wd, c, act, _stream())
+  if channel_weights is None:
+    _lib.call('edet_fuse_dw', arr, len(specs), _ptr(dw_w, torch.float32),
+              _ptr(out, torch.float16), n, h, wd, c, act, _stream())
+    return
+  if tuple(channel_weights.shape) != (len(specs), c):
+    raise ValueError('fuse_dw: channel_weights must be [%d, %d], got %s'
+                     % (len(specs), c, tuple(channel_weights.shape)))
+  _lib.call('edet_fuse_dw_channel', arr, len(specs), _ptr(channel_weights, torch.float32),
+            _ptr(dw_w, torch.float32), _ptr(out, torch.float16), n, h, wd, c, act, _stream())
 
 
 SEPCONV_MAX_C = 128   # edet_sepconv limits (c and nout)

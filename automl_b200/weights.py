@@ -90,7 +90,8 @@ def variable_specs(arch):
                                                             'sep_dw', True)
       s[node.op_scope + '/conv/pointwise_kernel'] = VarSpec((1, 1, f, f),
                                                             'sep_pw', True)
-      s[node.op_scope + '/conv/bias'] = VarSpec((f,), 'bias', True)
+      if not arch.conv_bn_act_pattern:   # use_bias=not conv_bn_act_pattern (:520)
+        s[node.op_scope + '/conv/bias'] = VarSpec((f,), 'bias', True)
       _bn(s, node.op_scope + '/bn', f)
 
   dets = ((('class', arch.num_classes * arch.num_anchors, 'class_bias'),

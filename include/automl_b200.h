@@ -212,6 +212,20 @@ typedef struct {
 int edet_fuse_dw(const edet_fuse_input* h_inputs, int n_inputs, const float* dw_w,
                  edet_half* out, int n, int h, int wd, int c, int act, edet_stream_t stream);
 
+/*
+ * edet_fuse_dw with one fusion weight per input AND channel: the channel_attn /
+ * channel_fastattn methods of fuse_features (efficientdet_arch.py:448-468,
+ * tf2/efficientdet_keras.py:101-115, 146-151), whose WSM variables have shape [c].
+ *   fuse_w float32 [n_inputs][c]: the normalised weights (per-channel softmax over the inputs, or
+ *   relu(w) / (sum relu + 1e-4)), computed on the host; edet_fuse_input.weight is ignored.
+ * fuse_w and dw_w are read before the kernel waits for the previous launch on the stream (PDL):
+ * neither may be written by that launch.  Same accumulation order as edet_fuse_dw: weights equal
+ * across the channels give its bits.
+ */
+int edet_fuse_dw_channel(const edet_fuse_input* h_inputs, int n_inputs, const float* fuse_w,
+                         const float* dw_w, edet_half* out, int n, int h, int wd, int c, int act,
+                         edet_stream_t stream);
+
 /* Fused separable convolution of a head tower layer (wgmma):
  *   out = post_act( pointwise( depthwise3x3( input ) ) + bias )
  * i.e. a depthwise conv followed by edet_pointwise_conv without the [n,h,w,c] intermediate in HBM
