@@ -28,6 +28,7 @@ static Option g_options[] = {
     {"pw_teams", 0, 3, {0}},         // 0 auto, 2 / 3 consumer warpgroups in pointwise_tc
     {"pw_smem_kb", 0, 227, {0}},     // 0 auto, else shared-memory budget of a pointwise_tc CTA
     {"persist_slack", 0, 132, {0}},  // CTAs a persistent kernel leaves out of its grid
+    {"max_ctas", 0, 4096, {0}},      // 0 no cap, else the grid of a persistent kernel (at most its work)
 };
 static Option* find_option(const char* name) {
   for (Option& o : g_options)
@@ -41,6 +42,7 @@ int option_sepconv_impl() { return option_value(2); }
 int option_pw_teams() { return option_value(3); }
 int option_pw_smem_kb() { return option_value(4); }
 int option_persist_slack() { return option_value(5); }
+int option_max_ctas() { return option_value(6); }
 
 int current_device() {
   int dev = -1;
@@ -64,6 +66,16 @@ int device_sm_count() {
     cached[dev].store(v, std::memory_order_relaxed);
   }
   return v;
+}
+
+int persistent_grid(int total_work, int ctas_per_sm) {
+  const int sms = device_sm_count();
+  if (!sms) return 0;
+  int grid = ctas_per_sm * sms - option_persist_slack();
+  const int cap = option_max_ctas();
+  if (cap && grid > cap) grid = cap;
+  if (grid > total_work) grid = total_work;
+  return grid < 1 ? 1 : grid;
 }
 
 namespace pwtc {

@@ -188,10 +188,16 @@ int option_stem_impl(); // 0 auto (tensor-core stem), 1 CUDA-core stem kernel
 int option_sepconv_impl();  // 0 auto (TMA-staged input for c <= 64, one buffer), 1 loads straight from global, 2 TMA double buffer
 int option_pw_teams();  // 0 auto, 2 / 3 = force that many epilogue teams in pointwise_tc
 int option_pw_smem_kb();     // 0 auto, else the shared-memory budget (KiB) of a pointwise_tc CTA
-int option_persist_slack();  // CTAs a persistent kernel leaves out of its two-per-SM grid (default 0)
+int option_persist_slack();  // CTAs a persistent kernel leaves out of its grid (default 0)
+int option_max_ctas();       // 0 (default): no cap, else the exact grid of a persistent kernel
 constexpr int kMaxDevices = 64;
 int current_device();                 // ordinal of the current device, -1 (+ error text) on failure
 int device_sm_count();                // multiprocessor count of the current device, 0 on failure
+// Grid of every persistent kernel: max(1, min(total_work, ctas_per_sm * sm_count - persist_slack,
+// max_ctas or unbounded)).  Never more CTAs than work items: a CTA whose first item does not exist
+// would never claim one, and the dynamic tile scheduler counts on every CTA retiring after a
+// claim.  0 (+ error text) when the SM count cannot be read.
+int persistent_grid(int total_work, int ctas_per_sm);
 // Opt a kernel into `bytes` of dynamic shared memory once per (kernel instantiation, device).
 // `done` is the caller's zero-initialised static int[kMaxDevices] (one per instantiation), so no
 // CUDA API call is made on the steady-state / graph-capture path.

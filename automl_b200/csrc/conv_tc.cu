@@ -50,6 +50,7 @@ struct Params {
   int desc_sbo;       // byte distance between 8-row groups in smem (8 * row pitch)
   int desc_layout;    // wgmma layout type: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B
   int ldr;
+  int no_odd_col, no_odd_row;   // stride 2 on a 1-wide / 1-high input: that sub-image is empty
   int total_tiles;
   const float* bias;
   const __half* residual;
@@ -125,6 +126,10 @@ conv_tc_kernel(const __grid_constant__ Maps maps, const Params p) {
             map_id = py * 2 + px;
             cy = tc.ty * TH + ((ry - py) >> 1);
             cx = tc.tx * TW + ((rx - px) >> 1);
+            // an empty sub-image has a stand-in map whose one column (row) is real memory: move
+            // the box off it, where TMA reads the zeros of the 'SAME' padding
+            if (px && p.no_odd_col) cx = -TW;
+            if (py && p.no_odd_row) cy = -TH;
           }
           const int s = team * p.team_stages + stage;
           mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
@@ -286,6 +291,8 @@ extern "C" int edet_conv2d(const edet_half* in, const edet_half* wt, const float
   p.a_stage_bytes = BLOCK_M * p.block_k * 2;
   p.b_stage_bytes = ((p.block_n * p.block_k * 2 + 1023) / 1024) * 1024;
   p.ldr = cout;
+  p.no_odd_col = stride == 2 && w == 1;
+  p.no_odd_row = stride == 2 && h == 1;
   p.bias = bias;
   p.residual = reinterpret_cast<const __half*>(residual);
   p.total_tiles = n * p.num_m_blocks * p.num_n_blocks;
@@ -310,7 +317,8 @@ extern "C" int edet_conv2d(const edet_half* in, const edet_half* wt, const float
     for (int py = 0; py < 2; ++py)
       for (int px = 0; px < 2; ++px) {
         // sub-image rows py, py+2, ... and columns px, px+2, ...; a 1-wide image has no odd column:
-        // give that map one (never addressed in bounds) column so that the encoder accepts it
+        // give that map one column so that the encoder accepts it (the producer never reads it:
+        // no_odd_col / no_odd_row move those boxes out of bounds)
         const int sh = (h - py + 1) / 2, sw = (w - px + 1) / 2;
         if ((rc = make_map4_strided(&maps.a[py * 2 + px], x + (static_cast<size_t>(py) * w + px) * cin,
                                     cin, sw > 0 ? sw : 1, sh > 0 ? sh : 1, n,
@@ -324,9 +332,8 @@ extern "C" int edet_conv2d(const edet_half* in, const edet_half* wt, const float
     return rc;
   if ((rc = make_map4(&maps.o, out, cout, p.wo, p.ho, n, kStoreCols, TW, TH))) return rc;
 
-  const int sm_count = device_sm_count();
-  if (!sm_count) return EDET_ERR_CUDA;
-  const int grid = p.total_tiles < sm_count ? p.total_tiles : sm_count;
+  const int grid = persistent_grid(p.total_tiles, 1);
+  if (!grid) return EDET_ERR_CUDA;
   const bool has_res = residual != nullptr;
   cudaStream_t s = as_stream(stream);
 #define EDET_CONV_CASE(A)                                                \

@@ -351,11 +351,8 @@ extern "C" int edet_conv2d_transpose(const edet_half* a0, int c0, int lda0, cons
                                   4ull * h * w * ldo, kStoreCols, TW, TH)))
         return rc;
 
-  const int sm_count = device_sm_count();
-  if (!sm_count) return EDET_ERR_CUDA;
-  int grid = sm_count - option_persist_slack();
-  if (grid < 1) grid = 1;
-  if (grid > p.total_tiles) grid = p.total_tiles;
+  const int grid = persistent_grid(p.total_tiles, 1);
+  if (!grid) return EDET_ERR_CUDA;
   cudaStream_t s = as_stream(stream);
   switch (act) {
     case EDET_ACT_NONE: return launch_nt<EDET_ACT_NONE>(maps, p, grid, smem_bytes, s);

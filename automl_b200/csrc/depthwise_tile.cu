@@ -310,11 +310,8 @@ static int run_ks(const __half* in, __half* out, const float* w, const float* bi
   if (!p.sched) return EDET_ERR_CUDA;
   CUtensorMap mx;
   if (int rc = make_map4(&mx, in, c, wd, h, n, kCB, C::TIW, C::TIH, /*swizzle=*/false)) return rc;
-  const int sms = device_sm_count();
-  if (!sms) return EDET_ERR_CUDA;
-  int grid = 2 * sms - option_persist_slack();
-  if (grid < sms) grid = sms;
-  if (p.total_units < grid) grid = p.total_units;
+  const int grid = persistent_grid(p.total_units, 2);
+  if (!grid) return EDET_ERR_CUDA;
   return launch_kernel<K, S>(mx, p, grid, act, stream);
 }
 

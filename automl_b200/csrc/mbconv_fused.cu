@@ -396,13 +396,12 @@ extern "C" int edet_mbconv_expand_dw(const edet_half* x, const edet_half* we, co
   if ((rc = make_map4(&mx, x, cin, w, h, n, p.block_k, kPatch, kPatch))) return rc;
   if ((rc = make_map(&mw, we, cin, cmid, 1, cin, static_cast<uint64_t>(cmid) * cin, p.ch, p.block_k)))
     return rc;
-  const int sm_count = device_sm_count();
-  if (!sm_count) return EDET_ERR_CUDA;
   // CTAs per SM the shared memory allows
   int per_sm = 232448 / (smem_bytes + 1024);
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 2) per_sm = 2;
-  const int grid = p.total_tiles < per_sm * sm_count ? p.total_tiles : per_sm * sm_count;
+  const int grid = persistent_grid(p.total_tiles, per_sm);
+  if (!grid) return EDET_ERR_CUDA;
   const bool has_se = se_sum != nullptr;
   cudaStream_t s = as_stream(stream);
   if (k == 3 && stride == 1) return launch<3, 1>(mx, mw, p, grid, smem_bytes, act, has_se, s);

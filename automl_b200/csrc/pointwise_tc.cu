@@ -25,6 +25,7 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <climits>
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -538,10 +539,9 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   EDET_CHECK_ARG(max_team_stages >= 2, "pointwise_tc: block_n %d leaves <2 pipeline stages per consumer",
                  p.block_n);
 
-  const int sm_count = device_sm_count();
-  if (!sm_count) return EDET_ERR_CUDA;
-  int grid = sm_count - option_persist_slack();
-  if (grid < 1) grid = 1;
+  // the grid before the work units are known; capped by their number below
+  int grid = persistent_grid(INT_MAX, 1);
+  if (!grid) return EDET_ERR_CUDA;
   // Work units.  With W resident and one k-block an M block's A tile serves every N tile (the
   // class head: all anchors of its rows).  A is held only while the M blocks alone still give
   // every CTA a unit: with fewer (the small class-head levels) the N tiles of an M block finish

@@ -444,8 +444,6 @@ extern "C" int edet_sepconv(const edet_fuse_input* h_inputs, int n_inputs, int p
   CUtensorMap mw;
   if (int rc = make_map(&mw, pw_wt, c, nout, 1, c, static_cast<uint64_t>(nout) * c, p.npad, 64))
     return rc;
-  const int sm_count = device_sm_count();
-  if (!sm_count) return EDET_ERR_CUDA;
   cudaStream_t s = as_stream(stream);
   p.sched = next_sched_slot();
   if (!p.sched) return EDET_ERR_CUDA;
@@ -456,7 +454,8 @@ extern "C" int edet_sepconv(const edet_fuse_input* h_inputs, int n_inputs, int p
   const int cap = 4;
   if (per_sm > cap) per_sm = cap;
   if (per_sm < 1) per_sm = 1;
-  const int grid = p.total_tiles < per_sm * sm_count ? p.total_tiles : per_sm * sm_count;
+  const int grid = persistent_grid(p.total_tiles, per_sm);
+  if (!grid) return EDET_ERR_CUDA;
   if (direct && p.katoms == 1 && option_sepconv_impl() != 1) {
     // c <= 64: the input tile comes through TMA, double buffered (sepconv_direct_tma_kernel)
     CUtensorMap mx;
@@ -466,7 +465,7 @@ extern "C" int edet_sepconv(const edet_fuse_input* h_inputs, int n_inputs, int p
     const int smem_tma = 1024 + kAtomBytesA + p.b_atom_bytes + nbuf * kInTileBytes + 128;
     int per = 232448 / (smem_tma + 1024);
     if (per > (nbuf == 1 ? 4 : 3)) per = nbuf == 1 ? 4 : 3;
-    const int grid_tma = p.total_tiles < per * sm_count ? p.total_tiles : per * sm_count;
+    const int grid_tma = persistent_grid(p.total_tiles, per);
 #define EDET_SEPC_TMA(POST)                                                                   \
   if (post_act == POST)                                                                       \
     return nbuf == 1 ? launch_direct_tma<POST, 1>(mw, mx, p, grid_tma, smem_tma, s)           \

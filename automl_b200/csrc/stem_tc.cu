@@ -235,12 +235,11 @@ int run(const float* in, __half* out, const __half* w, const float* bias, int n,
   p.total_tiles = static_cast<int>(total);
   p.sched = next_sched_slot();
   if (!p.sched) return EDET_ERR_CUDA;
-  const int sms = device_sm_count();
-  if (!sms) return EDET_ERR_CUDA;
   const int smem_bytes = 1024 + kABytes + kBBytes + 2 * kInPad * 4 + 32;
   int per_sm = 232448 / (smem_bytes + 1024);
   if (per_sm > 4) per_sm = 4;
-  const int grid = p.total_tiles < per_sm * sms ? p.total_tiles : per_sm * sms;
+  const int grid = persistent_grid(p.total_tiles, per_sm);
+  if (!grid) return EDET_ERR_CUDA;
   if (act == EDET_ACT_SWISH) return launch<EDET_ACT_SWISH>(p, grid, smem_bytes, stream);
   if (act == EDET_ACT_RELU6) return launch<EDET_ACT_RELU6>(p, grid, smem_bytes, stream);
   if (act == EDET_ACT_NONE) return launch<EDET_ACT_NONE>(p, grid, smem_bytes, stream);

@@ -66,7 +66,13 @@ const char* edet_last_error(void);
  * 162 KiB up with two consumers and from 226 KiB with three (the widest plan: 128 x 64 W tiles
  * streamed with A, nout 8192); a smaller budget refuses the shapes it cannot hold with
  * EDET_ERR_INVALID;
- * "persist_slack" = CTAs a persistent kernel leaves out of its grid (default 0). */
+ * "persist_slack" = CTAs a persistent kernel leaves out of its grid (default 0);
+ * "max_ctas" = 0 (default: no cap) | 1..4096: the most CTAs a persistent kernel launches.
+ * Every persistent kernel (pointwise / class arg-max, tiled depthwise, conv2d, conv2d_transpose,
+ * sepconv, tensor-core stem, mbconv_expand_dw) launches
+ *   max(1, min(work items, CTAs per SM * SM count - persist_slack, max_ctas or unbounded))
+ * CTAs, so max_ctas = G <= SM count pins the grid to exactly G on any GPU whenever there are at
+ * least G work items. */
 int edet_set_option(const char* name, int value);
 int edet_get_option(const char* name, int* value);
 /* Number of SMs / compute capability of the current device (major*10+minor). */

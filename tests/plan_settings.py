@@ -1,15 +1,15 @@
 """The option settings under which the pointwise GEMM (edet_pointwise_conv / edet_class_argmax) must
 give the bits of the default plan: three consumer warpgroups, smaller shared-memory budgets, and a
-pinned grid.  The grid is pinned with persist_slack = sm_count - G, so the plan a setting selects
-depends only on the shapes, not on which H100 runs the test; G = 1 makes one CTA wrap its work-unit
-ring and every stage ring many times."""
+pinned grid.  The grid is pinned with max_ctas = G, so the plan a setting selects depends only on
+the shapes, not on which H100 runs the test; G = 1 makes one CTA wrap its work-unit ring and every
+stage ring many times."""
 import torch
 
 from automl_b200._lib import EdetError
 
 GRIDS = (1, 3, 8, 33)
 SMEM_KB = (96, 128, 160, 192)
-# (option, value); ('grid', G) sets persist_slack = sm_count - G
+# (option, value); ('grid', G) sets max_ctas = G
 SETTINGS = [('pw_teams', 3)] + [('pw_smem_kb', kb) for kb in SMEM_KB] + [('grid', g) for g in GRIDS]
 # Every shape runs from this budget up with two consumers (include/automl_b200.h): 1 KiB alignment
 # + two 24 KiB stages (64 x 64 A + streamed 128 x 64 W) per consumer + one 16 KiB slab set per
@@ -29,17 +29,13 @@ def must_run(setting):
 
 
 def reset(ops):
-  for opt in ('pw_teams', 'pw_smem_kb', 'persist_slack'):
+  for opt in ('pw_teams', 'pw_smem_kb', 'persist_slack', 'max_ctas'):
     ops.set_option(opt, 0)
 
 
 def apply(ops, setting):
   name, value = setting
-  if name == 'grid':
-    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-    ops.set_option('persist_slack', sms - value)
-  else:
-    ops.set_option(name, value)
+  ops.set_option('max_ctas' if name == 'grid' else name, value)
 
 
 def run_under(ops, setting, launch):

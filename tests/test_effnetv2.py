@@ -61,7 +61,12 @@ def rel_l2(a, b):
 @pytest.mark.gpu
 @pytest.mark.parametrize('name,size,batch,tol', [('efficientnetv2-s', 96, 2, 2e-3),
                                                  ('efficientnetv2-b0', (64, 80), 2, 1e-3),
-                                                 ('efficientnet-b0', 64, 1, 1e-3)])
+                                                 ('efficientnet-b0', 64, 1, 1e-3),
+                                                 # the only place the fused-conv shapes of these
+                                                 # models meet the whole network
+                                                 ('efficientnetv2-b3', 96, 2, 2e-3),
+                                                 ('efficientnetv2-m', (64, 96), 2, 2e-3),
+                                                 ('efficientnetv2-l', 64, 2, 2e-3)])
 def test_backbone_parity_vs_oracle(name, size, batch, tol):
   """Every block output, the reduction endpoints and the 1x1 head feature map against the fp32
   oracle on the same seeded weights and inputs: relative L2 <= 1e-3 per tensor.  The 40-block

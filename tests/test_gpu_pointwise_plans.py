@@ -197,8 +197,8 @@ def test_pointwise_strided_operands(case, impl_name):
 # ---------------------------------------------------------------------------------------------
 def test_depthwise_tiled_persist_slack():
   """The TMA-tiled depthwise kernel is the other persistent kernel that leaves persist_slack CTAs
-  out of its grid (2 x sm_count - slack, at least sm_count, at most one CTA per work unit): output
-  bits and SE integers (per-unit sums, 2^-20 fixed point) must not depend on it."""
+  out of its grid (2 x sm_count - slack, at most one CTA per work unit) and whose grid max_ctas
+  pins: output bits and SE integers (per-unit sums, 2^-20 fixed point) must not depend on either."""
   ops = _ops()
   # 5x5 stride 1 runs on the tiled kernel when its 8 x 16 output tiles cover the map with <= 30 %
   # waste (dwt::eligible): 80 x 80 is covered exactly.  10 x 5 tiles x 11 64-channel slices = 550
@@ -209,20 +209,21 @@ def test_depthwise_tiled_persist_slack():
   wk = (torch.randn(k * k, c, generator=g) / k).to(DEV)
   bias = (torch.randn(c, generator=g) * 0.1).to(DEV)
   outs, sums = [], []
-  for slack in (0, 66, 132):
+  settings = [('persist_slack', v) for v in (0, 66, 132)] + [('max_ctas', g) for g in ps.GRIDS]
+  for opt, value in settings:
     out = torch.empty(n, h, w, c, dtype=torch.float16, device=DEV)
     part = torch.zeros(n, c, dtype=torch.int64, device=DEV)
     try:
-      ops.set_option('persist_slack', slack)
+      ops.set_option(opt, value)
       ops.depthwise_conv(x, out, wk, bias, utils.ACT_SWISH, k, s, part)
       torch.cuda.synchronize()
     finally:
-      ops.set_option('persist_slack', 0)
+      ops.set_option(opt, 0)
     outs.append(out)
     sums.append(part)
-  for i in (1, 2):
-    assert torch.equal(outs[i], outs[0])
-    assert torch.equal(sums[i], sums[0])
+  for i in range(1, len(settings)):
+    assert torch.equal(outs[i], outs[0]), settings[i]
+    assert torch.equal(sums[i], sums[0]), settings[i]
   # and the register-tiled kernel, which does the same fp32 arithmetic, gives the same output bits
   reg = torch.empty(n, h, w, c, dtype=torch.float16, device=DEV)
   try:
