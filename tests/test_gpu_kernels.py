@@ -181,7 +181,7 @@ def test_depthwise_conv(case):
   n, h, w, c, k, s, act, has_bias, has_se = case
   g = torch.Generator().manual_seed(99 + h + c + k)
   x = torch.randn(n, h, w, c, generator=g).half()
-  wk = (torch.randn(k, k, c, generator=g) / k).half()
+  wk = torch.randn(k, k, c, generator=g) / k              # genuine fp32 taps
   bias = torch.randn(c, generator=g) * 0.1 if has_bias else None
   ho, wo = -(-h // s), -(-w // s)
   out = torch.empty(n, ho, wo, c, dtype=torch.float16, device=DEV)
@@ -263,7 +263,7 @@ def test_mbconv_expand_dw(case):
   x = torch.randn(n, h, w, cin, generator=g).half()
   we = (torch.randn(cmid, cin, generator=g) / cin**0.5).half()
   be = torch.randn(cmid, generator=g) * 0.2
-  wk = (torch.randn(k, k, cmid, generator=g) / k).half()
+  wk = torch.randn(k, k, cmid, generator=g) / k           # genuine fp32 taps
   bd = torch.randn(cmid, generator=g) * 0.1
   ho, wo = -(-h // s), -(-w // s)
   out = torch.full((n, ho, wo, cmid), 7.0, dtype=torch.float16, device=DEV)
@@ -357,7 +357,7 @@ def test_fuse_dw_all_modes():
     up = torch.randn(n, uh, uw, c, generator=g).half()
     down = torch.randn(n, dh, dw, c, generator=g).half()
     wts = [0.5, 0.3, 0.2]
-    dwk = (torch.randn(3, 3, c, generator=g) / 3).half()
+    dwk = torch.randn(3, 3, c, generator=g) / 3              # genuine fp32 taps
     out = torch.empty(n, h, w, c, dtype=torch.float16, device=DEV)
     specs = [(same.to(DEV), ops.RS_SAME, None, wts[0]), (up.to(DEV), ops.RS_UP, None, wts[1]),
              (down.to(DEV), ops.RS_DOWN, (3, 3, 2, 2), wts[2])]
@@ -398,7 +398,7 @@ def test_fuse_dw_bifpn_signatures(sig, hw):
     modes = [(ops.RS_SAME, None), (ops.RS_DOWN, (3, 3, 2, 2))]
     res = [nchw(tens[0]), eo.max_pool_same(nchw(tens[1]), (3, 3), (2, 2))]
   wts = [0.45, 0.35, 0.2][:len(tens)]
-  dwk = (torch.randn(3, 3, c, generator=g) / 3).half()
+  dwk = torch.randn(3, 3, c, generator=g) / 3            # genuine fp32 taps
   out = torch.empty(n, h, w, c, dtype=torch.float16, device=DEV)
   specs = [(t.to(DEV), m, pool, wt) for t, (m, pool), wt in zip(tens, modes, wts)]
   ops.fuse_dw(specs, dwk.reshape(9, c).float().to(DEV), out, utils.ACT_SWISH)
