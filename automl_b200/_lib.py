@@ -62,6 +62,8 @@ SIGNATURES = {
                              c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     'edet_max_pool': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                               c_int, c_int, c_void_p]),
+    'edet_global_avg_pool': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    'edet_dense': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     'edet_pre_nms': (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p),
                              ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int, c_void_p,
                              c_void_p, c_void_p, c_void_p, c_int, c_void_p]),

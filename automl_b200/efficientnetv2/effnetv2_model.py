@@ -1,22 +1,29 @@
 """EfficientNet V1 / V2 backbone on the H100 path: the forward pass of the reference's
 efficientnetv2/effnetv2_model.py (`EffNetV2Model.call` :595-658) lowered to the C-ABI kernels.
 
+  model = effnetv2_model.get_model('efficientnetv2-s', include_top=True, weights=None,
+                                   batch_size=128, image_size=384)
+  logits = model(images)                         # float32 [N, 1000]
+  outs = model(images, with_endpoints=True)      # [logits, reduction_1, ..., reduction_5]
+
   model = effnetv2_model.get_model('efficientnetv2-s', weights=None, batch_size=128, image_size=384)
   features = model(images)                       # head_1x1 feature map, fp16 [N, h, w, 1280]
-  outs = model(images, with_endpoints=True)      # [head_1x1, reduction_1, ..., reduction_5]
 
 Mirrored: block-string configs, `round_filters` (:84-95, no 0.9 rule) / `round_repeats` (:98-102),
 block expansion (:541-566), `MBConvBlock` (:150-311), `FusedMBConvBlock` (:313-406, no SE in any
 registered model; expand_ratio == 1 blocks are ONE k x k conv followed by the activation),
 `SE` (:105-147), `Stem` (:409-432), the 1x1 head conv + BN + act (`Head` :435-470, endpoint
-'head_1x1'), residual rule (:270-277), endpoints 'reduction_i' (:616-637).  Out of scope (SURVEY.md
-row 21): global pooling + dropout + the classification `_fc`, pretrained-weight download,
-training (survival_prob / drop_connect are identities at inference).
+'head_1x1'), residual rule (:270-277), endpoints 'reduction_i' (:616-637) and, with
+include_top=True, the classification top: global average pooling (`Head.call` :477-496, endpoints
+'pooled_features' and 'head', float32; dropout is the identity at inference) and the Dense `_fc`
+(:571-578, :644-646), float32 from the pooled mean to the logits.  Out of scope: pretrained-weight
+download, training (dropout, survival_prob / drop_connect are identities at inference).
 
 Variable names follow the Keras layer names of the reference: <model>/stem/conv2d/kernel,
 <model>/blocks_<i>/{conv2d, conv2d_1, depthwise_conv2d, se/conv2d, se/conv2d_1,
 tpu_batch_normalization[_n]}, <model>/head/conv2d/kernel; the un-named BN layers of Stem / Head get
-Keras' default 'batch_normalization'.
+Keras' default 'batch_normalization', the un-named Dense layer 'dense' (<model>/dense/kernel
+[head_filters, num_classes], <model>/dense/bias).
 """
 import collections
 import math
@@ -60,7 +67,7 @@ class EffNetV2Arch(object):
   def __init__(self, model_name='efficientnetv2-s', model_config=None):
     cfg = effnetv2_configs.get_model_config(model_name)
     if model_config:
-      cfg.override(model_config)
+      cfg.model.override(model_config)    # the model section, as the reference does (:525)
     self.cfg = cfg
     m = self.mconfig = cfg.model
     self.model_name = model_name
@@ -90,8 +97,9 @@ class EffNetV2Arch(object):
                        if i == len(self.blocks) - 1 or self.blocks[i + 1].strides > 1]
 
 
-def variable_specs(arch):
-  """OrderedDict name -> VarSpec (Keras layouts) for the backbone + head conv."""
+def variable_specs(arch, include_top=False):
+  """OrderedDict name -> VarSpec (Keras layouts) for the backbone + head conv and, with include_top
+  and a non-zero num_classes (:572), the Dense classifier after them."""
   s = collections.OrderedDict()
   mn = arch.model_name
   s['%s/stem/conv2d/kernel' % mn] = VarSpec((3, 3, 3, arch.stem_filters), 'conv', True)
@@ -126,23 +134,24 @@ def variable_specs(arch):
   s['%s/head/conv2d/kernel' % mn] = VarSpec((1, 1, arch.blocks[-1].output_filters, arch.head_filters),
                                             'conv', True)
   _bn(s, '%s/head/batch_normalization' % mn, arch.head_filters)
+  if include_top and arch.mconfig.num_classes:
+    s['%s/dense/kernel' % mn] = VarSpec((arch.head_filters, arch.mconfig.num_classes), 'dense', True)
+    s['%s/dense/bias' % mn] = VarSpec((arch.mconfig.num_classes,), 'dense_bias', True)
   return s
 
 
 def count_params(arch, include_top=True):
   """Keras `model.count_params()` of the reference model: every variable above (BN moving
-  statistics included) plus, with include_top, the Dense classifier (effnetv2_model_test.py:25-48)."""
-  total = sum(int(np.prod(v.shape)) for v in variable_specs(arch).values())
-  if include_top and arch.mconfig.num_classes:
-    total += arch.head_filters * arch.mconfig.num_classes + arch.mconfig.num_classes
-  return total
+  statistics included) and, with include_top, the Dense classifier (effnetv2_model_test.py:25-48)."""
+  return sum(int(np.prod(v.shape)) for v in variable_specs(arch, include_top).values())
 
 
-def synthetic_weights(arch, seed=0):
-  """Seeded float32 weights keyed by variable name (no checkpoints offline)."""
+def synthetic_weights(arch, seed=0, include_top=False):
+  """Seeded float32 weights keyed by variable name (no checkpoints offline).  The Dense tensors
+  are drawn last, so the backbone of a seed has the same bits with and without the top."""
   rng = np.random.default_rng(seed)
   out = collections.OrderedDict()
-  for name, spec in variable_specs(arch).items():
+  for name, spec in variable_specs(arch, include_top).items():
     shape, kind = spec.shape, spec.kind
     if kind == 'conv':
       kh, kw, cin, _ = shape
@@ -157,6 +166,10 @@ def synthetic_weights(arch, seed=0):
       w = rng.normal(0.0, 0.1, size=shape)
     elif kind == 'var':
       w = rng.uniform(0.5, 1.5, size=shape)
+    elif kind == 'dense':          # N(0, 1/K): logits of O(1)
+      w = rng.normal(0.0, math.sqrt(1.0 / shape[0]), size=shape)
+    elif kind == 'dense_bias':     # the reference's constant (:576), perturbed so a wrong bias shows
+      w = (arch.mconfig.headbias or 0) + rng.normal(0.0, 0.1, size=shape)
     else:
       raise AssertionError(kind)
     out[name] = np.asarray(w, np.float32)
@@ -172,13 +185,16 @@ def _bn_fold(w, scope, eps):
 
 class EffNetV2Model(object):
   """One network instance bound to a device, a batch size and an image size (static buffers, the
-  forward pass is one CUDA graph).  There is no CPU fallback."""
+  forward pass is one CUDA graph).  There is no CPU fallback.
+
+  include_top=True adds the pooling and, when num_classes is non-zero, the Dense classifier: the
+  model returns float32 logits [N, num_classes] (the pooled features [N, C] when num_classes is 0).
+  include_top=False returns the fp16 'head_1x1' map; the reference returns the pooled tensor there,
+  which this path has never done and callers of the feature map rely on."""
 
   def __init__(self, model_name='efficientnetv2-s', model_config=None, include_top=False,
                weights=None, batch_size=1, image_size=None, device='cuda:0', use_cuda_graph=True,
                seed=0):
-    if include_top:
-      raise NotImplementedError('the classification head (pooling + Dense) is out of scope')
     if not torch.cuda.is_available():
       raise RuntimeError('EffNetV2Model needs a CUDA device; there is no CPU fallback')
     self.arch = a = EffNetV2Arch(model_name, model_config)
@@ -188,11 +204,18 @@ class EffNetV2Model(object):
     self.image_size = utils.parse_image_size(size)
     self.device = torch.device(device)
     self.use_cuda_graph = use_cuda_graph
+    self.include_top = bool(include_top)
     if weights is None:
-      weights = synthetic_weights(a, seed)
+      weights = synthetic_weights(a, seed, self.include_top)
     elif isinstance(weights, str):
       data = np.load(weights)
-      weights = {k: np.asarray(data[k], np.float32) for k in variable_specs(a)}
+      names = list(variable_specs(a, self.include_top))
+      missing = [k for k in names if k not in data.files]
+      if missing:
+        raise ValueError('%s lacks %d variables of %s%s: %s' % (
+            weights, len(missing), a.model_name, ' (include_top=True)' if self.include_top else '',
+            ', '.join(missing[:8]) + (', ...' if len(missing) > 8 else '')))
+      weights = {k: np.asarray(data[k], np.float32) for k in names}
     self.endpoints = {}
     self._ops, self.op_info, self._keep, self._graph = [], [], [], None
     with torch.cuda.device(self.device):
@@ -338,7 +361,26 @@ class EffNetV2Model(object):
     self._add('head_1x1', lambda x=x, head=head: ops.pointwise_conv(x, hw_[0], hb_, head, act),
               'pointwise_tc', nbytes=2 * (x.numel() + head.numel()),
               flops=2 * a.blocks[-1].output_filters * head.numel())
-    self.endpoints['head_1x1'] = head
+    self.endpoints['head_1x1'] = self.output = head
+    if not self.include_top:
+      return
+    # Head.call :477-496: global average pooling; dropout is the identity at inference, so 'head'
+    # is the pooled tensor.  local_pooling keeps the [N,1,1,C] shape of avg_pool until the Dense.
+    pooled = buf((n, a.head_filters), f32)
+    self._add('avg_pool', lambda: ops.global_avg_pool(head, pooled), 'global_avg_pool',
+              nbytes=2 * head.numel() + 4 * pooled.numel(), flops=head.numel())
+    view = pooled.view(n, 1, 1, -1) if a.mconfig.local_pooling else pooled
+    self.endpoints['pooled_features'] = self.endpoints['head'] = view
+    self.output = pooled
+    nc = a.mconfig.num_classes
+    if nc:                      # _build :571-578, call :644-646
+      fc_w = self._dev(np.asarray(w['%s/dense/kernel' % mn], np.float64).T, f16)   # [classes, K]
+      fc_b = self._dev(w['%s/dense/bias' % mn], f32)
+      logits = buf((n, nc), f32)
+      self._add('dense', lambda: ops.dense(pooled, fc_w, fc_b, logits), 'dense',
+                nbytes=2 * fc_w.numel() + 4 * (pooled.numel() + fc_b.numel() + logits.numel()),
+                flops=2 * fc_w.numel() * n)
+      self.output = logits
 
   # ---- execution ----------------------------------------------------------------------------
   def _run_ops(self):
@@ -360,8 +402,10 @@ class EffNetV2Model(object):
       self._graph.replay()
 
   def __call__(self, images=None, training=False, with_endpoints=False):
-    """images float32 [N,H,W,3] (already scaled to [-1,1], preprocessing.py:82-83) -> the
-    'head_1x1' feature map, or with_endpoints [head_1x1, reduction_1, ...] (:648-657)."""
+    """images float32 [N,H,W,3] (already scaled to [-1,1], preprocessing.py:82-83) -> the model
+    output `out`: float32 logits [N, num_classes] with include_top (pooled features [N, C] when
+    num_classes is 0), else the fp16 'head_1x1' feature map; with_endpoints [out, reduction_1,
+    ...] (:648-657)."""
     if training:
       raise NotImplementedError('inference only')
     if images is not None:
@@ -370,7 +414,7 @@ class EffNetV2Model(object):
         raise ValueError('expected input shape %s, got %s' % (tuple(self.input.shape), tuple(t.shape)))
       self.input.copy_(t.to(torch.float32), non_blocking=True)
     self.run()
-    out = self.endpoints['head_1x1']
+    out = self.output
     if with_endpoints:
       return [out] + [self.endpoints['reduction_%d' % i] for i in range(1, 6)
                       if 'reduction_%d' % i in self.endpoints]
@@ -379,17 +423,18 @@ class EffNetV2Model(object):
 
   def serve_stream(self, batches):
     """Pipelined __call__ over an iterable of host batches (float32 [N,H,W,3], ideally pinned):
-    the H2D copy of batch i+1 and the D2H copy of the feature map of batch i-1 overlap the network
+    the H2D copy of batch i+1 and the D2H copy of the output of batch i-1 overlap the network
     of batch i (two copy streams for the two PCIe directions, device staging buffers on both
-    sides).  Yields the 'head_1x1' feature map of each batch, in order, as a pinned host float16
-    tensor that stays valid until two further results have been yielded."""
+    sides).  Yields the model output of each batch (what __call__ returns: float32 logits with
+    include_top, else the float16 'head_1x1' feature map), in order, as a pinned host tensor
+    that stays valid until two further results have been yielded."""
     with torch.cuda.device(self.device):
       if getattr(self, '_pipe', None) is None:
-        head = self.endpoints['head_1x1']
+        result = self.output
         self._pipe = {
             'in': [torch.empty_like(self.input) for _ in range(2)],
-            'out': [torch.empty_like(head) for _ in range(2)],
-            'host': [torch.empty(tuple(head.shape), dtype=head.dtype).pin_memory() for _ in range(2)],
+            'out': [torch.empty_like(result) for _ in range(2)],
+            'host': [torch.empty(tuple(result.shape), dtype=result.dtype).pin_memory() for _ in range(2)],
             'h2d': torch.cuda.Stream(device=self.device), 'd2h': torch.cuda.Stream(device=self.device),
             'ev_h2d': [torch.cuda.Event() for _ in range(2)],
             'ev_in_free': [torch.cuda.Event() for _ in range(2)],
@@ -398,7 +443,7 @@ class EffNetV2Model(object):
         }
       p = self._pipe
       main = torch.cuda.current_stream(self.device)
-      head = self.endpoints['head_1x1']
+      result = self.output
       prev = None
       for k, batch in enumerate(batches):
         s = k % 2
@@ -414,7 +459,7 @@ class EffNetV2Model(object):
         p['ev_in_free'][s].record(main)
         self.run()
         main.wait_event(p['ev_d2h'][s])                  # result k-2 has left this staging buffer
-        p['out'][s].copy_(head, non_blocking=True)
+        p['out'][s].copy_(result, non_blocking=True)
         p['ev_out'][s].record(main)
         with torch.cuda.stream(p['d2h']):
           p['d2h'].wait_event(p['ev_out'][s])

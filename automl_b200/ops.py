@@ -237,7 +237,28 @@ def max_pool(x, out, pool, stride):
             pool[0], pool[1], stride[0], stride[1], _stream())
 
 
-CLASS_ARGMAX_COLS = 96   # columns per anchor of the padded class-head weights (edet_class_argmax)
+def global_avg_pool(x, out):
+  """x fp16 [N, ..., C] (NHWC map) -> out float32 [N, C], the mean over the pixels."""
+  n, c = x.shape[0], x.shape[-1]
+  if tuple(out.shape) != (n, c):
+    raise ValueError('global_avg_pool: out must be [%d, %d], got %s' % (n, c, tuple(out.shape)))
+  _lib.call('edet_global_avg_pool', _ptr(x, torch.float16), _ptr(out, torch.float32), n,
+            x.numel() // max(n * c, 1), c, _stream())
+
+
+def dense(x, wt, bias, out):
+  """x float32 [N, K], wt fp16 [num_classes, K], bias float32 [num_classes] -> out float32
+  [N, num_classes] = x @ wt^T + bias."""
+  n, k = x.shape
+  m = wt.shape[0]
+  if wt.shape[1] != k or tuple(bias.shape) != (m,) or tuple(out.shape) != (n, m):
+    raise ValueError('dense: x %s, wt %s, bias %s, out %s do not agree'
+                     % (tuple(x.shape), tuple(wt.shape), tuple(bias.shape), tuple(out.shape)))
+  _lib.call('edet_dense', _ptr(x, torch.float32), _ptr(wt, torch.float16),
+            _ptr(bias, torch.float32), _ptr(out, torch.float32), n, k, m, _stream())
+
+
+CLASS_ARGMAX_COLS = 96  # columns per anchor of the padded class-head weights (edet_class_argmax)
 
 
 def class_argmax(a, wt_padded, bias_padded, scores, classes, anchor_begin, num_anchors):

@@ -253,6 +253,28 @@ int edet_max_pool(const edet_half* in, edet_half* out, int n, int h, int wd, int
                   int pool_w, int stride_h, int stride_w, edet_stream_t stream);
 
 /*
+ * Global average pooling of an NHWC map: out[i, ch] = mean over the hw pixels of x[i, :, ch].
+ * Replaces GlobalAveragePooling2D / the whole-map tf.nn.avg_pool of the classifier head
+ * (efficientnetv2/effnetv2_model.py:477-492).
+ *   x half [n, hw, c] (c % 8 == 0, 16-byte aligned), out float32 [n, c]
+ * float32 accumulation in an order fixed by hw alone (no atomics): a row of `out` has the same
+ * bits for every n.
+ */
+int edet_global_avg_pool(const edet_half* x, float* out, int n, int hw, int c,
+                         edet_stream_t stream);
+
+/*
+ * Dense classifier on float32 features: out[i, j] = bias[j] + sum_k x[i, k] * wt[j, k].
+ * Replaces the `_fc` Dense layer (efficientnetv2/effnetv2_model.py:571-578, 644-646).
+ *   x float32 [n, k] (k % 8 == 0, 16-byte aligned), wt half [num_classes][k] (k contiguous),
+ *   bias float32 [num_classes], out float32 [n, num_classes] (dense rows, any num_classes >= 1)
+ * Nothing is rounded to half between the features and the logits; the sum over k runs in an
+ * order fixed by k alone, so a row of `out` has the same bits for every n.
+ */
+int edet_dense(const float* x, const edet_half* wt, const float* bias, float* out, int n, int k,
+               int num_classes, edet_stream_t stream);
+
+/*
  * Class-predict 1x1 convolution of ONE pyramid level fused with the class half of pre-NMS: the
  * [n, h, w, num_anchors * num_classes] logits are never written; per pixel and anchor the kernel
  * rounds each logit to fp16 (what edet_pointwise_conv would have stored), takes max / first
