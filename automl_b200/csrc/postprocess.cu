@@ -294,8 +294,9 @@ constexpr int kBCapB = 4096;
 constexpr int kBChunk = 64;         // candidates per chunk (8 lanes each)
 constexpr int kFastBins = 2048;
 
+// -0 takes +0's key: better() and TF's heap treat the two scores as equal (index order decides)
 __device__ __forceinline__ uint32_t score_key(float s) {
-  const uint32_t b = __float_as_uint(s);
+  const uint32_t b = s == 0.f ? 0u : __float_as_uint(s);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);  // monotone float -> uint
 }
 __device__ __forceinline__ float key_score(uint32_t k) {

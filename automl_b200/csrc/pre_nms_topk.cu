@@ -45,7 +45,10 @@ struct Smem {
   int sel_rank;
 };
 
+// -0 takes +0's key: tf.math.top_k compares the logits as floats, where the two are equal (a tie
+// that keeps the lower flat index)
 __device__ __forceinline__ unsigned key16(unsigned short h) {
+  h = h == 0x8000u ? static_cast<unsigned short>(0) : h;
   return (h & 0x8000u) ? (~static_cast<unsigned>(h) & 0xffffu) : (static_cast<unsigned>(h) | 0x8000u);
 }
 __device__ __forceinline__ unsigned short unkey16(unsigned k) {
