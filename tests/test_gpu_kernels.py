@@ -245,7 +245,7 @@ def test_depthwise_tiled_equals_register_kernel(case):
 # n, h, w, cin, cmid, k, stride, act, has_se   (D0 blocks 1-5 shapes at small sizes + edge cases)
 MBF_CASES = [
     (2, 40, 40, 16, 96, 3, 2, utils.ACT_SWISH, True),     # block 1: one chunk, 32B swizzle
-    (2, 33, 29, 24, 144, 3, 1, utils.ACT_SWISH, True),    # block 2: two chunks (80 + 64), K pad 24 -> 32
+    (2, 33, 29, 24, 144, 3, 1, utils.ACT_SWISH, True),    # block 2: three chunks of 48, K pad 24 -> 32
     (1, 37, 41, 24, 144, 5, 2, utils.ACT_SWISH, True),    # block 3
     (2, 20, 20, 40, 240, 5, 1, utils.ACT_SWISH, True),    # block 4: two k-blocks of 32
     (1, 23, 17, 40, 240, 3, 2, utils.ACT_RELU6, False),   # block 5 (lite flavour)
