@@ -33,12 +33,17 @@ import torch
 
 from automl_b200 import ops
 from automl_b200 import utils
+from automl_b200.backbone.efficientnet_builder import _layer_namer
 from automl_b200.efficientnetv2 import effnetv2_configs
+from automl_b200.lowering import LaunchList, bn_fold
 from automl_b200.weights import VarSpec, _bn
 
 Block = collections.namedtuple('Block', [
     'name', 'conv_type', 'kernel_size', 'strides', 'expand_ratio', 'input_filters',
-    'output_filters', 'mid_filters', 'se_filters', 'has_skip'])
+    'output_filters', 'mid_filters', 'se_filters', 'has_skip',
+    'expand_name', 'expand_bn',    # None when expand_ratio == 1
+    'dw_bn',                       # None for Fused-MBConv (conv_type 1)
+    'project_name', 'project_bn'])
 
 
 def round_filters(filters, mconfig, skip=False):
@@ -85,11 +90,17 @@ class EffNetV2Arch(object):
         has_se = ba.se_ratio is not None and 0 < ba.se_ratio <= 1
         # the reference sizes the SE bottleneck from the block's (rounded) input filters
         se = max(1, int(cin * ba.se_ratio)) if has_se else 0
+        # Keras layer names in creation order: expand conv + BN, depthwise BN, project conv + BN
+        conv, bn = _layer_namer('conv2d'), _layer_namer('tpu_batch_normalization')
+        expand_name, expand_bn = (conv(), bn()) if ba.expand_ratio != 1 else (None, None)
+        dw_bn = bn() if ba.conv_type == 0 else None
         self.blocks.append(Block(
             name='blocks_%d' % len(self.blocks), conv_type=ba.conv_type,
             kernel_size=ba.kernel_size, strides=stride, expand_ratio=ba.expand_ratio,
             input_filters=cin, output_filters=cout, mid_filters=cin * ba.expand_ratio,
-            se_filters=se, has_skip=(stride == 1 and cin == cout)))
+            se_filters=se, has_skip=(stride == 1 and cin == cout),
+            expand_name=expand_name, expand_bn=expand_bn, dw_bn=dw_bn,
+            project_name=conv(), project_bn=bn()))
         cin, stride = cout, 1
     self.head_filters = round_filters(m.feature_size or 1280, m)
     # a block is a reduction endpoint when it is last or the next block strides (:616-621)
@@ -106,28 +117,22 @@ def variable_specs(arch, include_top=False):
   _bn(s, '%s/stem/batch_normalization' % mn, arch.stem_filters)
   for b in arch.blocks:
     sc = '%s/%s' % (mn, b.name)
-    convs = iter(['conv2d', 'conv2d_1'])
-    bns = iter(['tpu_batch_normalization', 'tpu_batch_normalization_1', 'tpu_batch_normalization_2'])
-    if b.conv_type == 0:
-      if b.expand_ratio != 1:
-        s['%s/%s/kernel' % (sc, next(convs))] = VarSpec((1, 1, b.input_filters, b.mid_filters), 'conv', True)
-        _bn(s, '%s/%s' % (sc, next(bns)), b.mid_filters)
+    if b.expand_name:
+      ek = 1 if b.conv_type == 0 else b.kernel_size
+      s['%s/%s/kernel' % (sc, b.expand_name)] = VarSpec((ek, ek, b.input_filters, b.mid_filters), 'conv', True)
+      _bn(s, '%s/%s' % (sc, b.expand_bn), b.mid_filters)
+    if b.dw_bn:
       s['%s/depthwise_conv2d/depthwise_kernel' % sc] = VarSpec(
           (b.kernel_size, b.kernel_size, b.mid_filters, 1), 'dw', True)
-      _bn(s, '%s/%s' % (sc, next(bns)), b.mid_filters)
-    else:
-      if b.expand_ratio != 1:
-        s['%s/%s/kernel' % (sc, next(convs))] = VarSpec(
-            (b.kernel_size, b.kernel_size, b.input_filters, b.mid_filters), 'conv', True)
-        _bn(s, '%s/%s' % (sc, next(bns)), b.mid_filters)
+      _bn(s, '%s/%s' % (sc, b.dw_bn), b.mid_filters)
     if b.se_filters:
       s['%s/se/conv2d/kernel' % sc] = VarSpec((1, 1, b.mid_filters, b.se_filters), 'conv', True)
       s['%s/se/conv2d/bias' % sc] = VarSpec((b.se_filters,), 'se_bias', True)
       s['%s/se/conv2d_1/kernel' % sc] = VarSpec((1, 1, b.se_filters, b.mid_filters), 'conv', True)
       s['%s/se/conv2d_1/bias' % sc] = VarSpec((b.mid_filters,), 'se_bias', True)
     pk = b.kernel_size if (b.conv_type == 1 and b.expand_ratio == 1) else 1
-    s['%s/%s/kernel' % (sc, next(convs))] = VarSpec((pk, pk, b.mid_filters, b.output_filters), 'conv', True)
-    last_bn = '%s/%s' % (sc, next(bns))
+    s['%s/%s/kernel' % (sc, b.project_name)] = VarSpec((pk, pk, b.mid_filters, b.output_filters), 'conv', True)
+    last_bn = '%s/%s' % (sc, b.project_bn)
     _bn(s, last_bn, b.output_filters)
     # synthetic init only: a small gain on the residual branch keeps 40-100 stacked blocks O(1)
     s[last_bn + '/gamma'] = VarSpec((b.output_filters,), 'gamma_res' if b.has_skip else 'gamma', True)
@@ -176,14 +181,7 @@ def synthetic_weights(arch, seed=0, include_top=False):
   return out
 
 
-def _bn_fold(w, scope, eps):
-  g, b = np.asarray(w[scope + '/gamma'], np.float64), np.asarray(w[scope + '/beta'], np.float64)
-  m, v = np.asarray(w[scope + '/moving_mean'], np.float64), np.asarray(w[scope + '/moving_variance'], np.float64)
-  scale = g / np.sqrt(v + eps)
-  return scale, b - m * scale
-
-
-class EffNetV2Model(object):
+class EffNetV2Model(LaunchList):
   """One network instance bound to a device, a batch size and an image size (static buffers, the
   forward pass is one CUDA graph).  There is no CPU fallback.
 
@@ -202,7 +200,8 @@ class EffNetV2Model(object):
     self.n = int(batch_size)
     size = image_size or a.cfg.eval.isize
     self.image_size = utils.parse_image_size(size)
-    self.device = torch.device(device)
+    super().__init__(device)
+    self.act = a.act
     self.use_cuda_graph = use_cuda_graph
     self.include_top = bool(include_top)
     if weights is None:
@@ -217,27 +216,17 @@ class EffNetV2Model(object):
             ', '.join(missing[:8]) + (', ...' if len(missing) > 8 else '')))
       weights = {k: np.asarray(data[k], np.float32) for k in names}
     self.endpoints = {}
-    self._ops, self.op_info, self._keep, self._graph = [], [], [], None
+    self._graph = None
     with torch.cuda.device(self.device):
       self._build(weights)
 
   # ---- lowering -----------------------------------------------------------------------------
-  def _dev(self, arr, dtype):
-    t = torch.as_tensor(np.ascontiguousarray(arr)).to(dtype).to(self.device).contiguous()
-    self._keep.append(t)
-    return t
-
-  def _add(self, name, fn, kind, nbytes=0, flops=0):
-    self._ops.append((name, fn))
-    self.op_info.append({'name': name, 'kind': kind, 'bytes': int(nbytes), 'flops': int(flops)})
-
   def _build(self, w):
-    a, n, act, eps = self.arch, self.n, self.arch.act, self.arch.bn_eps
+    a, n, act, eps = self.arch, self.n, self.act, self.arch.bn_eps
     f16, f32 = torch.float16, torch.float32
     mn = a.model_name
     h, wd = self.image_size
-    buf = lambda shape, dt=f16: torch.empty(shape, dtype=dt, device=self.device)
-    self.input = buf((n, h, wd, 3), f32)
+    self.input = self._buf('input', (n, h, wd, 3), f32)
     for c in [a.stem_filters, a.head_filters] + [v for b in a.blocks for v in
                                                   (b.input_filters, b.mid_filters, b.output_filters)]:
       if c % 8:
@@ -245,111 +234,49 @@ class EffNetV2Model(object):
 
     def conv_w(name, scope_bn):
       """Conv2D kernel [kh,kw,Cin,Cout] with its BN folded -> ([taps, Cout, Cin] fp16, bias fp32)."""
-      s, sh = _bn_fold(w, scope_bn, eps)
+      s, sh = bn_fold(w, scope_bn, eps)
       k = np.asarray(w[name], np.float64) * s
       kh, kw, cin, cout = k.shape
       return self._dev(k.transpose(0, 1, 3, 2).reshape(kh * kw, cout, cin), f16), self._dev(sh, f32)
 
     # stem: conv3x3 s2 3 -> C + BN + act (Stem :409-432)
-    s, sh = _bn_fold(w, '%s/stem/batch_normalization' % mn, eps)
-    ks = np.asarray(w['%s/stem/conv2d/kernel' % mn], np.float64) * s
-    stem_w, stem_b = self._dev(ks.reshape(27, a.stem_filters), f16), self._dev(sh, f32)
     h, wd = -(-h // 2), -(-wd // 2)
-    x = buf((n, h, wd, a.stem_filters))
-    self._add('stem', lambda x=x: ops.stem_conv(self.input, x, stem_w, stem_b, act), 'stem',
-              nbytes=self.input.numel() * 4 + x.numel() * 2, flops=2 * 27 * x.numel())
+    x = self._stem(w, mn + '/stem/conv2d', mn + '/stem/batch_normalization', (h, wd))
     self.endpoints['stem'] = x
-
-    max_mid = max(b.mid_filters for b in a.blocks)
-    se_acc = [torch.zeros((n, max_mid), dtype=torch.int64, device=self.device) for _ in range(2)]
-    se_index = 0
-    if any(b.se_filters for b in a.blocks):
-      self._add('se_clear', lambda t=se_acc[0]: t.zero_(), 'memset')
+    self._se_accumulators(a.blocks)
     red = 0
     for bi, b in enumerate(a.blocks):
       sc = '%s/%s' % (mn, b.name)
-      x_in, s_ = x, b.strides
-      ho, wo = -(-h // s_), -(-wd // s_)
-      res = x_in if b.has_skip else None
-      y = buf((n, ho, wo, b.output_filters))
-      convs = iter(['conv2d', 'conv2d_1'])
-      bns = iter(['tpu_batch_normalization', 'tpu_batch_normalization_1', 'tpu_batch_normalization_2'])
-      if b.conv_type == 1:
+      if b.conv_type == 0:
+        y, (ho, wo) = self._mbconv(w, sc, b, x, (h, wd), b.strides)
+      else:
         if b.se_filters:
           raise NotImplementedError('Fused-MBConv with SE (no registered model has it)')
-        if b.expand_ratio != 1:
-          ew, eb = conv_w('%s/%s/kernel' % (sc, next(convs)), '%s/%s' % (sc, next(bns)))
-          mid = buf((n, ho, wo, b.mid_filters))
+        x_in, s_ = x, b.strides
+        ho, wo = -(-h // s_), -(-wd // s_)
+        res = x_in if b.has_skip else None
+        y = self._buf(b.name + '/out', (n, ho, wo, b.output_filters))
+        if b.expand_name:
+          ew, eb = conv_w('%s/%s/kernel' % (sc, b.expand_name), '%s/%s' % (sc, b.expand_bn))
+          mid = self._buf(b.name + '/expand_kxk', (n, ho, wo, b.mid_filters))
           self._add(b.name + '/expand_kxk',
                     lambda x_in=x_in, ew=ew, eb=eb, mid=mid, b=b:
                     ops.conv2d(x_in, ew, eb, mid, act, b.kernel_size, b.strides), 'conv_tc',
                     nbytes=2 * (x_in.numel() + mid.numel() + ew.numel()),
                     flops=2 * b.kernel_size**2 * b.input_filters * mid.numel())
-          pw, pb = conv_w('%s/%s/kernel' % (sc, next(convs)), '%s/%s' % (sc, next(bns)))
+          pw, pb = conv_w('%s/%s/kernel' % (sc, b.project_name), '%s/%s' % (sc, b.project_bn))
           self._add(b.name + '/project',
                     lambda mid=mid, pw=pw, pb=pb, y=y, res=res:
                     ops.pointwise_conv(mid, pw[0], pb, y, utils.ACT_NONE, residual=res),
                     'pointwise_tc', nbytes=2 * (mid.numel() + y.numel() * (2 if res is not None else 1)),
                     flops=2 * b.mid_filters * y.numel())
         else:   # ONE k x k conv + BN + act (+ skip)   (:355-364, :401-402)
-          pw, pb = conv_w('%s/%s/kernel' % (sc, next(convs)), '%s/%s' % (sc, next(bns)))
+          pw, pb = conv_w('%s/%s/kernel' % (sc, b.project_name), '%s/%s' % (sc, b.project_bn))
           self._add(b.name + '/conv_kxk',
                     lambda x_in=x_in, pw=pw, pb=pb, y=y, res=res, b=b:
                     ops.conv2d(x_in, pw, pb, y, act, b.kernel_size, b.strides, residual=res),
                     'conv_tc', nbytes=2 * (x_in.numel() + y.numel() * (2 if res is not None else 1)),
                     flops=2 * b.kernel_size**2 * b.input_filters * y.numel())
-      else:
-        mid = x_in
-        if b.expand_ratio != 1:
-          ew, eb = conv_w('%s/%s/kernel' % (sc, next(convs)), '%s/%s' % (sc, next(bns)))
-          mid = buf((n, h, wd, b.mid_filters))
-          self._add(b.name + '/expand',
-                    lambda x_in=x_in, ew=ew, eb=eb, mid=mid: ops.pointwise_conv(x_in, ew[0], eb, mid, act),
-                    'pointwise_tc', nbytes=2 * (x_in.numel() + mid.numel()),
-                    flops=2 * b.input_filters * mid.numel())
-        s, sh = _bn_fold(w, '%s/%s' % (sc, next(bns)), eps)
-        kd = np.asarray(w[sc + '/depthwise_conv2d/depthwise_kernel'], np.float64)[..., 0] * s
-        dw_w, dw_b = self._dev(kd.reshape(b.kernel_size**2, -1), f32), self._dev(sh, f32)   # fp32 taps
-        dwo = buf((n, ho, wo, b.mid_filters))
-        partial = next_zero = None
-        if b.se_filters:
-          partial = se_acc[se_index % 2].view(-1)[:n * b.mid_filters].view(n, b.mid_filters)
-          next_zero = se_acc[(se_index + 1) % 2]
-          se_index += 1
-        self._add(b.name + '/dw',
-                  lambda mid=mid, dwo=dwo, dw_w=dw_w, dw_b=dw_b, partial=partial, b=b:
-                  ops.depthwise_conv(mid, dwo, dw_w, dw_b, act, b.kernel_size, b.strides, partial),
-                  'depthwise', nbytes=2 * (mid.numel() + dwo.numel()),
-                  flops=2 * b.kernel_size**2 * dwo.numel())
-        s, sh = _bn_fold(w, '%s/%s' % (sc, next(bns)), eps)
-        kp = np.asarray(w['%s/%s/kernel' % (sc, next(convs))], np.float64)[0, 0] * s   # [Cmid, Cout]
-        proj_wt, proj_b = self._dev(kp.T, f16), self._dev(sh, f32)
-        if b.se_filters:
-          w1 = self._dev(np.asarray(w[sc + '/se/conv2d/kernel'], np.float64)[0, 0].T, f32)
-          b1 = self._dev(w[sc + '/se/conv2d/bias'], f32)
-          w2 = self._dev(np.asarray(w[sc + '/se/conv2d_1/kernel'], np.float64)[0, 0], f32)
-          b2 = self._dev(w[sc + '/se/conv2d_1/bias'], f32)
-          gate = buf((n, b.mid_filters), f32)
-          hidden = buf((n, b.se_filters), f32)
-          wt_scaled = buf((n, b.output_filters, b.mid_filters))
-          inv_hw = 1.0 / float(ho * wo)
-          self._add(b.name + '/se',
-                    lambda partial=partial, inv_hw=inv_hw, w1=w1, b1=b1, w2=w2, b2=b2, gate=gate,
-                    proj_wt=proj_wt, wt_scaled=wt_scaled, next_zero=next_zero, hidden=hidden:
-                    ops.se_fc(partial, inv_hw, w1, b1, w2, b2, gate, act, proj_wt, wt_scaled,
-                              next_zero, hidden), 'se_fc', nbytes=2 * wt_scaled.numel())
-          self._add(b.name + '/project',
-                    lambda dwo=dwo, wt_scaled=wt_scaled, proj_b=proj_b, y=y, res=res, ho=ho, wo=wo:
-                    ops.pointwise_conv(dwo, wt_scaled, proj_b, y, utils.ACT_NONE, residual=res,
-                                       batch=n, rows=ho * wo), 'pointwise_tc',
-                    nbytes=2 * (dwo.numel() + y.numel() * (2 if res is not None else 1) + wt_scaled.numel()),
-                    flops=2 * b.mid_filters * y.numel())
-        else:
-          self._add(b.name + '/project',
-                    lambda dwo=dwo, proj_wt=proj_wt, proj_b=proj_b, y=y, res=res:
-                    ops.pointwise_conv(dwo, proj_wt, proj_b, y, utils.ACT_NONE, residual=res),
-                    'pointwise_tc', nbytes=2 * (dwo.numel() + y.numel() * (2 if res is not None else 1)),
-                    flops=2 * b.mid_filters * y.numel())
       x, h, wd = y, ho, wo
       self.endpoints['block_%d' % bi] = y
       if bi in a.reductions:
@@ -357,7 +284,7 @@ class EffNetV2Model(object):
         self.endpoints['reduction_%d' % red] = y
     self.endpoints['features'] = x
     hw_, hb_ = conv_w('%s/head/conv2d/kernel' % mn, '%s/head/batch_normalization' % mn)
-    head = buf((n, h, wd, a.head_filters))
+    head = self._buf('head_1x1', (n, h, wd, a.head_filters))
     self._add('head_1x1', lambda x=x, head=head: ops.pointwise_conv(x, hw_[0], hb_, head, act),
               'pointwise_tc', nbytes=2 * (x.numel() + head.numel()),
               flops=2 * a.blocks[-1].output_filters * head.numel())
@@ -366,7 +293,7 @@ class EffNetV2Model(object):
       return
     # Head.call :477-496: global average pooling; dropout is the identity at inference, so 'head'
     # is the pooled tensor.  local_pooling keeps the [N,1,1,C] shape of avg_pool until the Dense.
-    pooled = buf((n, a.head_filters), f32)
+    pooled = self._buf('avg_pool', (n, a.head_filters), f32)
     self._add('avg_pool', lambda: ops.global_avg_pool(head, pooled), 'global_avg_pool',
               nbytes=2 * head.numel() + 4 * pooled.numel(), flops=head.numel())
     view = pooled.view(n, 1, 1, -1) if a.mconfig.local_pooling else pooled
@@ -376,7 +303,7 @@ class EffNetV2Model(object):
     if nc:                      # _build :571-578, call :644-646
       fc_w = self._dev(np.asarray(w['%s/dense/kernel' % mn], np.float64).T, f16)   # [classes, K]
       fc_b = self._dev(w['%s/dense/bias' % mn], f32)
-      logits = buf((n, nc), f32)
+      logits = self._buf('dense', (n, nc), f32)
       self._add('dense', lambda: ops.dense(pooled, fc_w, fc_b, logits), 'dense',
                 nbytes=2 * fc_w.numel() + 4 * (pooled.numel() + fc_b.numel() + logits.numel()),
                 flops=2 * fc_w.numel() * n)

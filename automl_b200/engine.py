@@ -22,20 +22,11 @@ from automl_b200 import anchors as anchors_lib
 from automl_b200 import ops
 from automl_b200 import utils
 from automl_b200.arch import DetArch
+from automl_b200.lowering import LaunchList, bn_fold
 
 
 def _round_up(x, m):
   return (x + m - 1) // m * m
-
-
-def _bn_fold(w, scope, eps):
-  """(scale, shift) float64 for y = x*scale + shift."""
-  g = np.asarray(w[scope + '/gamma'], np.float64)
-  b = np.asarray(w[scope + '/beta'], np.float64)
-  m = np.asarray(w[scope + '/moving_mean'], np.float64)
-  v = np.asarray(w[scope + '/moving_variance'], np.float64)
-  scale = g / np.sqrt(v + eps)
-  return scale, b - m * scale
 
 
 def nms_v5_params(nms_configs):
@@ -55,7 +46,7 @@ def nms_v5_params(nms_configs):
   return iou_thresh, score_thresh, sigma / 2
 
 
-class Engine(object):
+class Engine(LaunchList):
   """One network instance bound to one device, one batch size and one image size."""
 
   def __init__(self, config, weights, batch_size, device='cuda:0', pw_impl=ops.PW_TCGEN05,
@@ -67,7 +58,7 @@ class Engine(object):
     self.config = config
     self.arch = a = DetArch(config)
     self.n = int(batch_size)
-    self.device = torch.device(device)
+    super().__init__(device)
     self.pw_impl = pw_impl
     self.use_cuda_graph = use_cuda_graph
     self.image_id_base = image_id_base
@@ -94,52 +85,11 @@ class Engine(object):
     self._logits_current = False   # the head output buffers hold the latest pass (forward())
     self.act = utils.activation_code(a.act_type)
     self._graph = None
-    self._bb_split = None
     self._cell0_end = None
-    self._ops = []          # (name, callable)
-    self.op_info = []       # parallel to _ops: kind / algorithmic bytes / flops
-    self._branch = None
     self._branch_streams = {}
-    self.buffers = {}       # debug / tests: name -> tensor
-    self._keep = []         # keeps weight tensors alive
     self.launches_per_forward = 0
     with torch.cuda.device(self.device):
       self._build(weights)
-
-  # ---- helpers --------------------------------------------------------------------------
-  def _dev(self, arr, dtype):
-    t = torch.as_tensor(np.ascontiguousarray(arr)).to(dtype).to(self.device).contiguous()
-    self._keep.append(t)
-    return t
-
-  def _buf(self, name, shape, dtype=torch.float16):
-    t = torch.empty(shape, dtype=dtype, device=self.device)
-    self.buffers[name] = t
-    return t
-
-  def _add(self, name, fn, kind='other', nbytes=0, flops=0, kernels=1, branch=None, needs=None):
-    """kind groups launches of the same kernel; nbytes / flops are the ALGORITHMIC HBM bytes
-    and floating-point operations of the launch (SURVEY.md 8d formulas), used by bench.py."""
-    self._ops.append((name, fn))
-    if branch is None:
-      branch = self._branch      # set while lowering independent sub-graphs (the head towers)
-    self.op_info.append({'name': name, 'kind': kind, 'bytes': int(nbytes), 'flops': int(flops),
-                         'kernels': int(kernels), 'branch': branch, 'needs': list(needs or [])})
-
-  def _pw(self, name, a, wt, bias, out, act, residual=None, batch=1, rows=None, nout=None,
-          branch=None):
-    if rows is None:
-      rows = a.numel() // (a.shape[-1] * batch)
-    impl = self.pw_impl
-    k = wt.shape[-1]
-    n_out = nout if nout is not None else wt.shape[-2]
-    m = rows * batch
-    wbatch = wt.shape[0] if wt.dim() == 3 else 1
-    nbytes = 2 * (m * k + m * n_out * (2 if residual is not None else 1)) + 2 * wbatch * n_out * k
-    self._add(name, lambda: ops.pointwise_conv(a, wt, bias, out, act, residual=residual,
-                                               rows=rows, batch=batch, nout=nout, impl=impl),
-              kind='pointwise_tc' if impl == ops.PW_TCGEN05 else 'pointwise_simt',
-              nbytes=nbytes, flops=2 * m * k * n_out, branch=branch)
 
   # ---- network lowering -------------------------------------------------------------------
   def _build(self, w):
@@ -153,124 +103,33 @@ class Engine(object):
       if c % 8:
         raise NotImplementedError('%s has %d channels; the kernels need multiples of 8' % (what, c))
 
-    # -- stem ---------------------------------------------------------------------------------
+    # -- stem and MBConv blocks ----------------------------------------------------------------
     bb = a.backbone_name
-    scale, shift = _bn_fold(w, bb + '/stem/tpu_batch_normalization', eps)
-    k = np.asarray(w[bb + '/stem/conv2d/kernel'], np.float64) * scale  # [3,3,3,C]
-    stem_w = self._dev(k.reshape(27, -1), f16)
-    stem_b = self._dev(shift, f32)
-    h, wd = a.level_hw[1]
-    x = self._buf('stem', (n, h, wd, a.stem_filters))
-    inp = self.input
-    self._add('stem', lambda inp=inp, x=x: ops.stem_conv(inp, x, stem_w, stem_b, act),
-              kind='stem', nbytes=12 * n * H * W + 2 * n * h * wd * a.stem_filters,
-              flops=2 * 27 * n * h * wd * a.stem_filters)
-    cur, cur_hw = x, (h, wd)
-
-    # -- MBConv blocks ----------------------------------------------------------------------
+    cur = self._stem(w, bb + '/stem/conv2d', bb + '/stem/tpu_batch_normalization', a.level_hw[1])
+    cur_hw = a.level_hw[1]
+    self._se_accumulators(a.blocks)
     feats = {}
-    max_mid = max(b.mid_filters for b in a.blocks)
-    se_acc = [self._buf('se_acc%d' % i, (n, max_mid), torch.int64) for i in range(2)]
-    for t in se_acc:
-      t.zero_()
-    se_index = 0
-    if any(b.se_filters for b in a.blocks):
-      # one explicit clear per forward keeps the ping-pong valid for any number of SE blocks
-      self._add('se_clear', lambda t=se_acc[0]: t.zero_(), kind='memset', nbytes=8 * n * max_mid,
-                kernels=0)   # torch fill kernel, not one of ours
     for b in a.blocks:
       scope = '%s/%s' % (bb, b.name)
       check_c(b.input_filters, scope); check_c(b.mid_filters, scope); check_c(b.output_filters, scope)
       h, wd = cur_hw
-      x_in = cur
-      mid = x_in
       # fuse_mbconv_front: blocks whose expanded map is large and whose depthwise is 3x3 stride 2
       # run the fused front half (expand in registers, depthwise from shared memory; the expanded map
       # never reaches HBM).  Off by default since round 2: with the three-team pointwise kernel
       # and the TMA-tiled depthwise the separate pair is 1 % faster on the D0 step (4.165 vs
       # 4.204 ms) although it moves 4x the bytes -- the fused kernel serialises TMA -> MMA ->
       # epilogue -> depthwise inside a CTA at two CTAs per SM (DESIGN.md section 4).
-      fuse_front = (self.fuse_mbconv_front and b.expand_name and b.kernel_size == 3 and
-                    b.stride == 2 and b.input_filters <= 64 and h * wd >= 1600)
-      exp_wt = exp_b = None
-      if b.expand_name:
-        s, sh = _bn_fold(w, '%s/%s' % (scope, b.expand_bn), eps)
-        kw = np.asarray(w['%s/%s/kernel' % (scope, b.expand_name)], np.float64)[0, 0]  # [Cin,Cmid]
-        exp_wt = self._dev((kw * s).T, f16)
-        exp_b = self._dev(sh, f32)
-        if not fuse_front:
-          mid = self._buf(b.name + '/expand', (n, h, wd, b.mid_filters))
-          self._pw(b.name + '/expand', x_in, exp_wt, exp_b, mid, act)
-      # depthwise
-      s, sh = _bn_fold(w, '%s/%s' % (scope, b.dw_bn), eps)
-      kd = np.asarray(w[scope + '/depthwise_conv2d/depthwise_kernel'], np.float64)[..., 0]  # [k,k,C]
-      dw_w = self._dev((kd * s).reshape(b.kernel_size * b.kernel_size, -1), f32)   # fp32 taps
-      dw_b = self._dev(sh, f32)
-      ho, wo = utils.same_pad(h, b.kernel_size, b.stride)[0], utils.same_pad(wd, b.kernel_size, b.stride)[0]
-      dwo = self._buf(b.name + '/dw', (n, ho, wo, b.mid_filters))
-      partial = None
-      if b.se_filters:
-        # int64 fixed-point squeeze accumulator [n, mid]; two buffers alternate between blocks,
-        # each block's se_fc launch clears the one the next block will accumulate into.
-        partial = se_acc[se_index % 2].view(-1)[:n * b.mid_filters].view(n, b.mid_filters)
-        next_zero = se_acc[(se_index + 1) % 2]
-        se_index += 1
-      if fuse_front:
-        self._add(b.name + '/expand_dw',
-                  lambda x_in=x_in, exp_wt=exp_wt, exp_b=exp_b, dwo=dwo, dw_w=dw_w, dw_b=dw_b,
-                  partial=partial, b=b:
-                  ops.mbconv_expand_dw(x_in, exp_wt, exp_b, dw_w, dw_b, dwo, act, b.kernel_size,
-                                       b.stride, partial),
-                  kind='mbconv_expand_dw',
-                  nbytes=2 * n * (h * wd * b.input_filters + ho * wo * b.mid_filters)
-                  + 2 * b.mid_filters * (b.input_filters + b.kernel_size**2)
-                  + (8 * partial.numel() if partial is not None else 0),
-                  flops=2 * n * b.mid_filters * (h * wd * b.input_filters + b.kernel_size**2 * ho * wo))
-      else:
-        self._add(b.name + '/dw',
-                  lambda mid=mid, dwo=dwo, dw_w=dw_w, dw_b=dw_b, partial=partial, b=b:
-                  ops.depthwise_conv(mid, dwo, dw_w, dw_b, act, b.kernel_size, b.stride, partial),
-                  kind='depthwise_k%ds%d' % (b.kernel_size, b.stride),
-                  nbytes=2 * n * b.mid_filters * (h * wd + ho * wo) + 2 * b.kernel_size**2 * b.mid_filters
-                  + (8 * partial.numel() if partial is not None else 0),
-                  flops=2 * b.kernel_size**2 * n * b.mid_filters * ho * wo)
-      # project (+SE folded into per-image weights, + skip)
-      s, sh = _bn_fold(w, '%s/%s' % (scope, b.project_bn), eps)
-      kp = np.asarray(w['%s/%s/kernel' % (scope, b.project_name)], np.float64)[0, 0]  # [Cmid,Cout]
-      proj_wt = self._dev((kp * s).T, f16)  # [Cout, Cmid]
-      proj_b = self._dev(sh, f32)
-      y = self._buf(b.name + '/out', (n, ho, wo, b.output_filters))
-      res = x_in if b.has_skip else None
-      if b.reduction and b.reduction >= a.config.min_level and self._bb_split is None:
-        # first op that writes a backbone feature the feature network reads (see run())
-        self._bb_split = len(self._ops) + (1 if b.se_filters else 0)
-      if b.se_filters:
-        w1 = self._dev(np.asarray(w[scope + '/se/conv2d/kernel'], np.float64)[0, 0].T, f32)   # [se,C]
-        b1 = self._dev(w[scope + '/se/conv2d/bias'], f32)
-        w2 = self._dev(np.asarray(w[scope + '/se/conv2d_1/kernel'], np.float64)[0, 0], f32)  # [se,C]
-        b2 = self._dev(w[scope + '/se/conv2d_1/bias'], f32)
-        gate = self._buf(b.name + '/se_gate', (n, b.mid_filters), f32)
-        hidden = self._buf(b.name + '/se_hidden', (n, b.se_filters), f32)
-        wt_scaled = self._buf(b.name + '/proj_w', (n, b.output_filters, b.mid_filters))
-        inv_hw = 1.0 / float(ho * wo)
-        self._add(b.name + '/se',
-                  lambda partial=partial, inv_hw=inv_hw, w1=w1, b1=b1, w2=w2, b2=b2, gate=gate,
-                  proj_wt=proj_wt, wt_scaled=wt_scaled, next_zero=next_zero, hidden=hidden:
-                  ops.se_fc(partial, inv_hw, w1, b1, w2, b2, gate, act, proj_wt, wt_scaled,
-                            next_zero, hidden),
-                  kind='se_fc', nbytes=8 * partial.numel() + 2 * proj_wt.numel() + 2 * wt_scaled.numel(),
-                  kernels=2)
-        self._pw(b.name + '/project', dwo, wt_scaled, proj_b, y, utils.ACT_NONE, residual=res,
-                 batch=n, rows=ho * wo)
-      else:
-        self._pw(b.name + '/project', dwo, proj_wt, proj_b, y, utils.ACT_NONE, residual=res)
-      cur, cur_hw = y, (ho, wo)
+      fuse_front = bool(self.fuse_mbconv_front and b.expand_name and b.kernel_size == 3 and
+                        b.stride == 2 and b.input_filters <= 64 and h * wd >= 1600)
+      cur, cur_hw = self._mbconv(w, scope, b, cur, cur_hw, b.stride, fuse_front)
       if b.reduction:
-        feats[b.reduction] = y
+        feats[b.reduction] = cur
 
     self.num_backbone_ops = len(self._ops)
-    if self._bb_split is None:
-      self._bb_split = self.num_backbone_ops
+    # first op that writes a backbone feature the feature network reads (see run())
+    first = next((b for b in a.blocks if b.reduction and b.reduction >= a.config.min_level), None)
+    self._bb_split = (self.op_names().index(first.name + '/project') if first else
+                      self.num_backbone_ops)
     if self.defer_heads:
       # the held-back head stage reads copies of P3..P5 (see _run_pipelined); torch's copy kernel
       for level in sorted(feats):
@@ -293,7 +152,7 @@ class Engine(object):
       kw = np.asarray(w[r.scope + '/conv2d/kernel'], np.float64)[0, 0]  # [Cin,F]
       cb = np.asarray(w[r.scope + '/conv2d/bias'], np.float64)
       if a.config.apply_bn_for_resampling:
-        s, sh = _bn_fold(w, r.scope + '/bn', eps)
+        s, sh = bn_fold(w, r.scope + '/bn', eps)
       else:
         s, sh = np.ones(F), np.zeros(F)
       wt = self._dev((kw * s).T, f16)
@@ -411,7 +270,7 @@ class Engine(object):
           specs.append((src, mode_code[mode], pool, float(wgt)))
         op = node.op_scope
         dw_w = self._dev(np.asarray(w[op + '/conv/depthwise_kernel'], np.float64)[..., 0].reshape(9, F), f32)
-        s, sh = _bn_fold(w, op + '/bn', eps)
+        s, sh = bn_fold(w, op + '/bn', eps)
         kp = np.asarray(w[op + '/conv/pointwise_kernel'], np.float64)[0, 0]
         cb = 0.0 if a.conv_bn_act_pattern else np.asarray(w[op + '/conv/bias'], np.float64)
         pw_wt = self._dev((kp * s).T, f16)
@@ -476,7 +335,7 @@ class Engine(object):
         ping = self._buf('%s/l%d/a' % (scope, level), (n, hh, ww, F))
         pong = self._buf('%s/l%d/b' % (scope, level), (n, hh, ww, F))
         for i in range(a.head_repeats):
-          s, sh = _bn_fold(w, '%s/%s-%d-bn-%d' % (scope, net, i, level), eps)
+          s, sh = bn_fold(w, '%s/%s-%d-bn-%d' % (scope, net, i, level), eps)
           wt = self._dev((pws[i] * s).T, f16)
           bias = self._dev(pbs[i] * s + sh, f32)
           y = ping if i % 2 == 0 else pong
@@ -621,7 +480,7 @@ class Engine(object):
     for st in a.seg_stages:
       kernel = np.asarray(w[st.kernel_scope + '/kernel'], np.float64)   # [3, 3, out, in]
       if st.bn_scope:
-        scale, bias = _bn_fold(w, st.bn_scope, a.bn_eps)
+        scale, bias = bn_fold(w, st.bn_scope, a.bn_eps)
         act = self.act
       else:
         scale, bias = None, np.asarray(w[st.kernel_scope + '/bias'], np.float64)

@@ -2,7 +2,7 @@
 
   * every tensor the engine writes to HBM rounded to fp16 (`Oracle(store=fp16_store)`), and
   * the GEMM weights the engine uploads: inference BatchNorm folded into the 1x1 / stem kernels in
-    float64, THEN rounded to fp16 (`engine.py::_bn_fold` + `_dev(..., f16)`); depthwise taps and
+    float64, THEN rounded to fp16 (`lowering.py::bn_fold` + `_dev(..., f16)`); depthwise taps and
     biases stay fp32, as on the device.
 
 All arithmetic stays fp32 on the CPU.  The difference between this model and the plain fp32
@@ -83,7 +83,7 @@ def device_weights(arch, w, round_gemm_weights=True):
 
 
 def effnetv2_device_weights(arch, w):
-  """The same for the EfficientNet V1 / V2 backbone (efficientnetv2/effnetv2_model.py::_build): BN
+  """The same for the EfficientNet V1 / V2 backbone (EffNetV2Model._build, lowering.py): BN
   folded into fp16 conv kernels (1x1 and k x k), fp32 depthwise taps."""
   out = dict(w)
   mn, eps = arch.model_name, arch.bn_eps
@@ -102,13 +102,11 @@ def effnetv2_device_weights(arch, w):
   fold(mn + '/stem/conv2d/kernel', mn + '/stem/batch_normalization')
   for b in arch.blocks:
     sc = '%s/%s' % (mn, b.name)
-    convs = iter(['conv2d', 'conv2d_1'])
-    bns = iter(['tpu_batch_normalization', 'tpu_batch_normalization_1', 'tpu_batch_normalization_2'])
-    if b.expand_ratio != 1:
-      fold('%s/%s/kernel' % (sc, next(convs)), '%s/%s' % (sc, next(bns)))
-    if b.conv_type == 0:
-      fold(sc + '/depthwise_conv2d/depthwise_kernel', '%s/%s' % (sc, next(bns)), depthwise=True)
-    fold('%s/%s/kernel' % (sc, next(convs)), '%s/%s' % (sc, next(bns)))
+    if b.expand_name:
+      fold('%s/%s/kernel' % (sc, b.expand_name), '%s/%s' % (sc, b.expand_bn))
+    if b.dw_bn:
+      fold(sc + '/depthwise_conv2d/depthwise_kernel', '%s/%s' % (sc, b.dw_bn), depthwise=True)
+    fold('%s/%s/kernel' % (sc, b.project_name), '%s/%s' % (sc, b.project_bn))
   fold(mn + '/head/conv2d/kernel', mn + '/head/batch_normalization')
   return out
 
