@@ -31,6 +31,8 @@ SIGNATURES = {
     'edet_set_option': (c_int, [ctypes.c_char_p, c_int]),
     'edet_get_option': (c_int, [ctypes.c_char_p, ctypes.POINTER(c_int)]),
     'edet_device_info': (c_int, [ctypes.POINTER(c_int), ctypes.POINTER(c_int)]),
+    'edet_sched_bind': (c_int, [c_void_p, c_int]),
+    'edet_last_sched_slot': (c_int, [ctypes.POINTER(c_void_p)]),
     'edet_preprocess': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                 ctypes.POINTER(c_float), ctypes.POINTER(c_float),
                                 ctypes.POINTER(c_float), c_void_p]),

@@ -1,4 +1,4 @@
-// Library-wide entry points: version, error text, device info.
+// Library-wide entry points: version, error text, device info, scheduler-slot binding.
 #include <stdarg.h>
 #include <string.h>
 
@@ -82,23 +82,40 @@ namespace pwtc {
 // zero-initialised in every context that loads the module; each slot resets itself
 __device__ unsigned g_tile_sched[2 * kSchedSlots];
 
-unsigned* next_sched_slot() {
+// The calling thread's binding (edet_sched_bind): the next slot to hand out and how many are
+// left; and the slot of its most recent slot-using launch (edet_last_sched_slot).
+static thread_local unsigned* t_bound_next = nullptr;
+static thread_local int t_bound_left = 0;
+static thread_local unsigned* t_last_slot = nullptr;
+
+int next_sched_slot(unsigned** slot) {
+  if (t_bound_next != nullptr) {
+    if (t_bound_left == 0) {
+      set_error("scheduler slots: every slot bound by edet_sched_bind is in use; nothing launched");
+      return EDET_ERR_INVALID;
+    }
+    *slot = t_last_slot = t_bound_next;
+    t_bound_next += 2;
+    --t_bound_left;
+    return EDET_OK;
+  }
   static std::atomic<unsigned*> base[kMaxDevices];
   static std::atomic<unsigned> next[kMaxDevices];
   const int dev = current_device();
-  if (dev < 0) return nullptr;
+  if (dev < 0) return EDET_ERR_CUDA;
   unsigned* b = base[dev].load(std::memory_order_acquire);
   if (b == nullptr) {
     void* addr = nullptr;
     if (cudaGetSymbolAddress(&addr, g_tile_sched) != cudaSuccess || addr == nullptr) {
       set_error("cudaGetSymbolAddress(g_tile_sched) failed");
-      return nullptr;
+      return EDET_ERR_CUDA;
     }
     b = static_cast<unsigned*>(addr);
     base[dev].store(b, std::memory_order_release);
   }
   const unsigned i = next[dev].fetch_add(1u, std::memory_order_relaxed) % kSchedSlots;
-  return b + 2 * i;
+  *slot = t_last_slot = b + 2 * i;
+  return EDET_OK;
 }
 }  // namespace pwtc
 }  // namespace edet
@@ -132,6 +149,20 @@ extern "C" int edet_get_option(const char* name, int* value) {
   return EDET_OK;
 }
 extern "C" const char* edet_last_error(void) { return edet::g_err; }
+extern "C" int edet_sched_bind(void* slots, int count) {
+  using namespace edet;
+  EDET_CHECK_ARG(slots == nullptr || count > 0, "sched_bind: count must be > 0 (got %d)", count);
+  EDET_CHECK_ARG(reinterpret_cast<uintptr_t>(slots) % 8 == 0, "sched_bind: slots must be 8-byte aligned");
+  pwtc::t_bound_next = static_cast<unsigned*>(slots);
+  pwtc::t_bound_left = slots ? count : 0;
+  return EDET_OK;
+}
+extern "C" int edet_last_sched_slot(void** slot) {
+  using namespace edet;
+  EDET_CHECK_ARG(slot != nullptr, "last_sched_slot: null pointer");
+  *slot = pwtc::t_last_slot;
+  return EDET_OK;
+}
 extern "C" int edet_device_info(int* sm_count, int* cc) {
   int dev = 0, sms = 0, major = 0, minor = 0;
   EDET_CHECK_CUDA(cudaGetDevice(&dev));

@@ -306,8 +306,7 @@ static int run_ks(const __half* in, __half* out, const float* w, const float* bi
   EDET_CHECK_ARG(total < 0x7fffffffLL, "depthwise(tile): too many work units");
   p.total_units = static_cast<int>(total);
   p.wgt = w; p.bias = bias; p.out = out; p.se_sum = se_sum;
-  p.sched = next_sched_slot();
-  if (!p.sched) return EDET_ERR_CUDA;
+  if (int rc = next_sched_slot(&p.sched)) return rc;
   CUtensorMap mx;
   if (int rc = make_map4(&mx, in, c, wd, h, n, kCB, C::TIW, C::TIH, /*swizzle=*/false)) return rc;
   const int grid = persistent_grid(p.total_units, 2);

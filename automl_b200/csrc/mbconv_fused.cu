@@ -388,8 +388,7 @@ extern "C" int edet_mbconv_expand_dw(const edet_half* x, const edet_half* we, co
   p.wd = wd;
   p.out = reinterpret_cast<__half*>(out);
   p.se_sum = reinterpret_cast<long long*>(se_sum);
-  p.sched = next_sched_slot();
-  if (!p.sched) return EDET_ERR_CUDA;
+  if (int rc = next_sched_slot(&p.sched)) return rc;
   EDET_CHECK_ARG(smem_bytes <= 232448, "mbconv_expand_dw: tile needs %d bytes of smem", smem_bytes);
   CUtensorMap mx, mw;
   int rc;

@@ -496,8 +496,7 @@ int run(const __half* a, int lda, const __half* wt, int wbatch, const float* bia
   p.ldr = ldr;
   p.bias = bias;
   p.residual = residual;
-  p.sched = next_sched_slot();
-  if (!p.sched) return EDET_ERR_CUDA;
+  if (int rc = next_sched_slot(&p.sched)) return rc;
 
   // every column the epilogue can touch: whole N tiles (n_valid is rounded up to 16 inside a tile)
   const int bias_cols = p.num_n_blocks * p.block_n;

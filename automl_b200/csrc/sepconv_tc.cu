@@ -445,8 +445,7 @@ extern "C" int edet_sepconv(const edet_fuse_input* h_inputs, int n_inputs, int p
   if (int rc = make_map(&mw, pw_wt, c, nout, 1, c, static_cast<uint64_t>(nout) * c, p.npad, 64))
     return rc;
   cudaStream_t s = as_stream(stream);
-  p.sched = next_sched_slot();
-  if (!p.sched) return EDET_ERR_CUDA;
+  if (int rc = next_sched_slot(&p.sched)) return rc;
   const bool direct = n_inputs == 1 && p.fuse.in[0].mode == EDET_RS_SAME &&
                       p.fuse.in[0].weight == 1.0f && pre_act == EDET_ACT_NONE;
   const int smem_bytes = 1024 + p.katoms * (kAtomBytesA + p.b_atom_bytes) + 64;

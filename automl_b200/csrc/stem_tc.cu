@@ -233,8 +233,7 @@ int run(const float* in, __half* out, const __half* w, const float* bias, int n,
   const long long total = static_cast<long long>(n) * p.tiles_x * p.tiles_y;
   EDET_CHECK_ARG(total < 0x7fffffffLL, "stem: too many tiles");
   p.total_tiles = static_cast<int>(total);
-  p.sched = next_sched_slot();
-  if (!p.sched) return EDET_ERR_CUDA;
+  if (int rc = next_sched_slot(&p.sched)) return rc;
   const int smem_bytes = 1024 + kABytes + kBBytes + 2 * kInPad * 4 + 32;
   int per_sm = 232448 / (smem_bytes + 1024);
   if (per_sm > 4) per_sm = 4;

@@ -296,7 +296,8 @@ __device__ __forceinline__ int sched_next_tile(unsigned* sched, int total_tiles)
   if (t >= total_tiles) sched_retire(sched);   // this CTA's last fetch
   return t;
 }
-// Pool of self-resetting scheduler counters, one pool per device (defined in capi.cu).
+// Global pool of self-resetting scheduler counters for unbound launches, one pool per device
+// (defined in capi.cu; see next_sched_slot).
 constexpr int kSchedSlots = 4096;
 // ---- host side ------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -318,12 +319,19 @@ inline EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// A scheduler slot ({next tile, finished CTAs} counter pair) for one launch, from the CURRENT
-// device's pool, handed out round robin with an atomic index: launches that may run concurrently
-// (parallel graph branches, several engines) get distinct slots as long as fewer than kSchedSlots
-// launches are alive at once; the address is baked into the graph node.  nullptr (+ error text)
-// on failure.  Defined in capi.cu.
-unsigned* next_sched_slot();
+// The scheduler slot ({next tile, finished CTAs} counter pair) of one launch, stored to *slot.
+// Two launches that run at the same time must never share a slot: both would claim from one
+// counter and skip tiles, and the slot could be left dirty for every later launch.  A captured
+// graph keeps the address for as long as it lives.
+//   - bound (edet_sched_bind on the calling thread): the next of the caller's consecutive slots;
+//     EDET_ERR_INVALID once they are used up.  The caller owns them and guarantees that two
+//     launches holding the same slot are never in flight together (the launch lists of
+//     lowering.py give each op its own slot);
+//   - unbound: the CURRENT device's global pool of kSchedSlots, round robin, so a slot comes back
+//     kSchedSlots launches later -- fine for standalone launches, not for graphs that live on.
+// Records the slot for edet_last_sched_slot.  EDET_OK or an error code (+ text).  Defined in
+// capi.cu.
+int next_sched_slot(unsigned** slot);
 
 // 3-D half tensor [d2][d1][d0] (d0 contiguous), box [1][box1][64], 128B swizzle.
 inline int make_map(CUtensorMap* map, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2,

@@ -34,6 +34,7 @@ class LaunchList(object):
     self._keep = []         # keeps weight tensors alive
     self.buffers = {}       # debug / tests: name -> tensor
     self._branch = None
+    self._sched_slots = None   # int32 [ops, 2]: the tile-scheduler slot of each op (_bound)
 
   def _dev(self, arr, dtype):
     t = torch.as_tensor(np.ascontiguousarray(arr)).to(dtype).to(self.device).contiguous()
@@ -48,11 +49,39 @@ class LaunchList(object):
   def _add(self, name, fn, kind='other', nbytes=0, flops=0, kernels=1, branch=None, needs=None):
     """kind groups launches of the same kernel; nbytes / flops are the ALGORITHMIC HBM bytes
     and floating-point operations of the launch (SURVEY.md 8d formulas), used by bench.py."""
-    self._ops.append((name, fn))
+    if self._sched_slots is not None:
+      raise RuntimeError('%s: the launch list has run; it takes no more ops' % name)
+    i = len(self._ops)
+    self._ops.append((name, lambda: self._bound(i, fn)))
     if branch is None:
       branch = self._branch      # set while lowering independent sub-graphs (the head towers)
     self.op_info.append({'name': name, 'kind': kind, 'bytes': int(nbytes), 'flops': int(flops),
                          'kernels': int(kernels), 'branch': branch, 'needs': list(needs or [])})
+
+  def _bound(self, i, fn):
+    """Runs op i with its scheduler-slot launch (if it makes one) on the list's slot i
+    (edet_sched_bind), not on the global pool, where a slot comes back 4096 launches later.
+
+    Op i then uses the same slot in the eager passes and in every graph that contains it, which
+    is safe because one op of one list is never in flight twice: the graphs and eager passes that
+    share ops are ordered on one stream (Engine: net, net+pre, bb1, bb2 and featcopy on the main
+    stream; cell0 and heads+pre on the head stream, over ops the main-stream stages of the
+    pipelined step do not run; forward()
+    waits for a pending head stage first), and a side stream of a parallel branch forks from and
+    joins back into its stream within the pass.  Lists never share slots with each other or
+    with standalone ops.* launches."""
+    pool = self._sched_slots
+    if pool is None:
+      if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError('a launch list must run eagerly once before it is captured')
+      pool = torch.zeros(len(self._ops), 2, dtype=torch.int32, device=self.device)
+      torch.cuda.synchronize(self.device)   # zero before any stream of the list uses a slot
+      self._sched_slots = pool
+    ops.sched_bind(pool.data_ptr() + 8 * i, 1)
+    try:
+      fn()
+    finally:
+      ops.sched_bind(None)
 
   def _pw(self, name, a, wt, bias, out, act, residual=None, batch=1, rows=None, nout=None,
           branch=None):

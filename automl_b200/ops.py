@@ -44,6 +44,20 @@ def get_option(name):
   return v.value
 
 
+def sched_bind(slots, count=0):
+  """Binds the calling thread's slot-using launches to `count` consecutive scheduler slots at
+  device address `slots` (2 * count zeroed uint32); None unbinds (see edet_sched_bind)."""
+  _lib.call('edet_sched_bind', ctypes.c_void_p(slots) if slots else None, int(count))
+
+
+def last_sched_slot():
+  """Device address of the scheduler slot of this thread's latest slot-using launch (0 before
+  the first)."""
+  v = ctypes.c_void_p()
+  _lib.call('edet_last_sched_slot', ctypes.byref(v))
+  return v.value or 0
+
+
 def preprocess(raw, out, mean_rgb, stddev_rgb):
   """raw uint8 [N,h,w,3] -> out fp32 [N,H,W,3]; returns image_scale_to_original (float)."""
   n, h, w, _ = raw.shape

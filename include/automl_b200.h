@@ -79,6 +79,24 @@ int edet_get_option(const char* name, int* value);
 int edet_device_info(int* sm_count, int* cc);
 
 /*
+ * Tile-scheduler slots.  The persistent kernels with a dynamic tile scheduler (pointwise conv and
+ * class arg-max, sepconv, the tiled depthwise kernel, the tensor-core stem, mbconv_expand_dw) claim
+ * work from a device counter pair, the launch's "slot", whose address a captured graph keeps.  Two
+ * launches in flight at the same time must not share a slot: both would skip tiles, silently.
+ *
+ * edet_sched_bind: from now on the slot-using launches made by the CALLING THREAD take consecutive
+ * slots of `slots` (device memory of 2 * count zeroed uint32 on the device they run on; every
+ * launch resets its slot when it finishes); the launch after the count-th is refused with
+ * EDET_ERR_INVALID and nothing is launched.  The caller guarantees that no two launches holding
+ * one slot are ever in flight together.  slots = NULL unbinds: launches then take slots round
+ * robin from a global pool of 4096 per device, so a slot is shared again 4096 launches later.
+ * edet_last_sched_slot: the slot of the calling thread's most recent slot-using launch (also set
+ * while a stream is being captured into a graph); NULL before the first.
+ */
+int edet_sched_bind(void* slots, int count);
+int edet_last_sched_slot(void** slot);
+
+/*
  * Serving pre-process: uint8 HWC images (all the same size) -> normalise -> aspect-preserving
  * bilinear resize (TF2 half-pixel centres) -> zero pad to [out_h, out_w].
  * Replaces inference.image_preprocess inference.py:37-56 and
