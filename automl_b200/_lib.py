@@ -15,6 +15,7 @@ c_void_p, c_int, c_float, c_size_t = (ctypes.c_void_p, ctypes.c_int, ctypes.c_fl
 RS_SAME, RS_UP, RS_DOWN = 0, 1, 2
 PW_TCGEN05, PW_SIMT = 0, 1
 NMS_HARD, NMS_DIOU, NMS_GAUSSIAN, NMS_LINEAR = 0, 1, 2, 3
+CLS_BILINEAR, CLS_BICUBIC = 0, 1
 
 
 class FuseInput(ctypes.Structure):
@@ -66,6 +67,9 @@ SIGNATURES = {
                               c_int, c_int, c_void_p]),
     'edet_global_avg_pool': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     'edet_dense': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    'edet_cls_preprocess': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                    c_void_p]),
+    'edet_softmax_topk': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     'edet_pre_nms': (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p),
                              ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int, c_void_p,
                              c_void_p, c_void_p, c_void_p, c_int, c_void_p]),

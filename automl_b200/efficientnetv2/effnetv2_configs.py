@@ -1,7 +1,8 @@
 """Model configs of the reference's efficientnetv2/effnetv2_configs.py (block-string grammar
 :25-93, V1 table :96-136, V2 tables :139-231) and the `model` section of hparams.base_config
 (efficientnetv2/hparams.py:221-243).  Only what the inference forward pass reads is kept; the
-train / data / eval sections keep the image sizes."""
+train / eval sections keep the image sizes, the data section the eval pre-process recipe
+(`augname`: 'effnetv1_*' selects the legacy bicubic recipe, preprocessing.py:133)."""
 import re
 
 from automl_b200.hparams_config import Config
@@ -59,16 +60,17 @@ v2_l_block = ['r4_k3_s1_e1_i32_o32_c1', 'r7_k3_s2_e4_i32_o64_c1', 'r7_k3_s2_e4_i
 v2_xl_block = ['r4_k3_s1_e1_i32_o32_c1', 'r8_k3_s2_e4_i32_o64_c1', 'r8_k3_s2_e4_i64_o96_c1',
                'r16_k3_s2_e4_i96_o192_se0.25', 'r24_k3_s1_e6_i192_o256_se0.25',
                'r32_k3_s2_e6_i256_o512_se0.25', 'r8_k3_s1_e6_i512_o640_se0.25']
-# (block, width, depth, train_size, eval_size, dropout)
+# (block, width, depth, train_size, eval_size, dropout, augname); the reference's randaug /
+# mixup magnitudes only matter for training and are not kept
 efficientnetv2_params = {
-    'efficientnetv2-s': (v2_s_block, 1.0, 1.0, 300, 384, 0.2),
-    'efficientnetv2-m': (v2_m_block, 1.0, 1.0, 384, 480, 0.3),
-    'efficientnetv2-l': (v2_l_block, 1.0, 1.0, 384, 480, 0.4),
-    'efficientnetv2-xl': (v2_xl_block, 1.0, 1.0, 384, 512, 0.4),
-    'efficientnetv2-b0': (v2_base_block, 1.0, 1.0, 192, 224, 0.2),
-    'efficientnetv2-b1': (v2_base_block, 1.0, 1.1, 192, 240, 0.2),
-    'efficientnetv2-b2': (v2_base_block, 1.1, 1.2, 208, 260, 0.3),
-    'efficientnetv2-b3': (v2_base_block, 1.2, 1.4, 240, 300, 0.3),
+    'efficientnetv2-s': (v2_s_block, 1.0, 1.0, 300, 384, 0.2, 'randaug'),
+    'efficientnetv2-m': (v2_m_block, 1.0, 1.0, 384, 480, 0.3, 'randaug'),
+    'efficientnetv2-l': (v2_l_block, 1.0, 1.0, 384, 480, 0.4, 'randaug'),
+    'efficientnetv2-xl': (v2_xl_block, 1.0, 1.0, 384, 512, 0.4, 'randaug'),
+    'efficientnetv2-b0': (v2_base_block, 1.0, 1.0, 192, 224, 0.2, 'effnetv1_autoaug'),
+    'efficientnetv2-b1': (v2_base_block, 1.0, 1.1, 192, 240, 0.2, 'effnetv1_autoaug'),
+    'efficientnetv2-b2': (v2_base_block, 1.1, 1.2, 208, 260, 0.3, 'effnetv1_autoaug'),
+    'efficientnetv2-b3': (v2_base_block, 1.2, 1.4, 240, 300, 0.3, 'effnetv1_autoaug'),
 }
 
 
@@ -86,15 +88,17 @@ def efficientnetv1_config(model_name='efficientnet-b0'):
   model = base_model_config()
   model.update(model_name=model_name, blocks_args=BlockDecoder().decode(v1_b0_block_str),
                width_coefficient=width, depth_coefficient=depth, dropout_rate=dropout)
-  return Config(dict(model=model, eval=dict(isize=isize), train=dict(isize=0.8)))
+  return Config(dict(model=model, eval=dict(isize=isize), train=dict(isize=0.8),
+                     data=dict(augname='effnetv1_autoaug')))
 
 
 def efficientnetv2_config(model_name='efficientnetv2-s'):
-  block, width, depth, train_size, eval_size, dropout = efficientnetv2_params[model_name]
+  block, width, depth, train_size, eval_size, dropout, aug = efficientnetv2_params[model_name]
   model = base_model_config()
   model.update(model_name=model_name, blocks_args=BlockDecoder().decode(block),
                width_coefficient=width, depth_coefficient=depth, dropout_rate=dropout)
-  return Config(dict(model=model, eval=dict(isize=eval_size), train=dict(isize=train_size)))
+  return Config(dict(model=model, eval=dict(isize=eval_size), train=dict(isize=train_size),
+                     data=dict(augname=aug)))
 
 
 def get_model_config(model_name):

@@ -272,6 +272,38 @@ def dense(x, wt, bias, out):
             _ptr(bias, torch.float32), _ptr(out, torch.float32), n, k, m, _stream())
 
 
+CLS_BILINEAR, CLS_BICUBIC = _lib.CLS_BILINEAR, _lib.CLS_BICUBIC
+CLS_DESC_WORDS = 8      # int32 words of one edet_cls_image row: offset (2 words), h, w, y0, x0, crop_h, crop_w
+SOFTMAX_TOPK_MAX_K = 32
+
+
+def cls_preprocess(images, desc, out, mode, bicubic_table=None):
+  """Classification eval pre-process of a (ragged) request in one launch: images uint8 (every image
+  packed back to back, HWC), desc int32 [N, 8] edet_cls_image rows (byte offset into `images`, h,
+  w, crop window; the caller keeps every window inside `images`), out float32 [N, S, S, 3]; mode
+  CLS_BILINEAR, or CLS_BICUBIC with bicubic_table float32 [2050] (see edet_cls_preprocess)."""
+  n, s = out.shape[0], out.shape[1]
+  if tuple(out.shape) != (n, s, s, 3) or tuple(desc.shape) != (n, CLS_DESC_WORDS):
+    raise ValueError('cls_preprocess: out %s must be [N, S, S, 3] and desc %s [N, %d]'
+                     % (tuple(out.shape), tuple(desc.shape), CLS_DESC_WORDS))
+  if mode == CLS_BICUBIC and (bicubic_table is None or bicubic_table.numel() != 2050):
+    raise ValueError('cls_preprocess: the bicubic mode needs the float32 [2050] coefficient table')
+  _lib.call('edet_cls_preprocess', _ptr(images, torch.uint8), _ptr(desc, torch.int32), n, s, mode,
+            _ptr(bicubic_table, torch.float32), _ptr(out, torch.float32), _stream())
+
+
+def softmax_topk(logits, probs, classes):
+  """logits float32 [N, C] -> probs float32 [N, k], classes int32 [N, k]: the k largest logits by
+  (logit descending, class ascending) and their softmax probabilities, 1 <= k <= min(C, 32)."""
+  n, c = logits.shape
+  k = probs.shape[1] if probs.dim() == 2 else -1
+  if tuple(probs.shape) != (n, k) or tuple(classes.shape) != (n, k):
+    raise ValueError('softmax_topk: probs %s and classes %s must be [%d, k]'
+                     % (tuple(probs.shape), tuple(classes.shape), n))
+  _lib.call('edet_softmax_topk', _ptr(logits, torch.float32), n, c, k, _ptr(probs, torch.float32),
+            _ptr(classes, torch.int32), _stream())
+
+
 CLASS_ARGMAX_COLS = 96  # columns per anchor of the padded class-head weights (edet_class_argmax)
 
 

@@ -293,6 +293,44 @@ int edet_dense(const float* x, const edet_half* wt, const float* bias, float* ou
                int num_classes, edet_stream_t stream);
 
 /*
+ * Classification eval pre-process of the EfficientNet V1 / V2 models: per image, a crop window of
+ * a uint8 HWC image -> resize to size x size -> normalise, in one launch for a ragged request.
+ * Replaces preprocessing.preprocess_image(image, size, is_training=False, augname=...)
+ * (efficientnetv2/preprocessing.py:58-70, 131-157; preprocess_legacy.py:110-127, 184-244).
+ *   images  uint8, every image packed back to back (HWC, 3 channels)
+ *   desc    DEVICE edet_cls_image [n]: byte offset of the image in `images`, its h and w, and the
+ *           crop window (y0, x0, crop_h, crop_w) the host computed (the whole image when not
+ *           cropping)
+ *   mode    EDET_CLS_BILINEAR: tf.image.resize bilinear (half-pixel centres), then (x - 128) / 128
+ *           EDET_CLS_BICUBIC:  TF1 resize_bicubic (no half-pixel centres, TF's CPU kernel), then
+ *                              (x - mean) / stddev, ImageNet mean / stddev * 255 in float32
+ *   bicubic_table  DEVICE float32 [2 * 1025]: TF's coefficient table (a = -0.75, 1024 steps;
+ *           entry i: t[2i] = ((a+2)x - (a+3))x^2 + 1, t[2i+1] = ((a(x+1) - 5a)(x+1) + 8a)(x+1) - 4a
+ *           with x = i / 1024, evaluated in double, stored as float); NULL for EDET_CLS_BILINEAR
+ *   out     float32 [n, size, size, 3]
+ * Every operation is a single IEEE float32 rounding in the reference's order (no contraction).
+ */
+typedef struct {
+  int64_t offset;
+  int32_t h, w, y0, x0, crop_h, crop_w;
+} edet_cls_image;
+#define EDET_CLS_BILINEAR 0
+#define EDET_CLS_BICUBIC 1
+int edet_cls_preprocess(const uint8_t* images, const edet_cls_image* desc, int n, int size,
+                        int mode, const float* bicubic_table, float* out, edet_stream_t stream);
+
+/*
+ * Softmax + top-k of classifier logits: per row, the k largest logits ordered by (logit
+ * descending, class index ascending) -- tf.math.top_k's tie rule -- and their softmax
+ * probabilities exp(l - max) / sum_j exp(l_j - max) (accurate expf, IEEE division).  The max and
+ * the sum run in an order fixed by num_classes alone: a row has the same bits for every n.
+ *   logits float32 [n, num_classes]; probs float32 [n, k]; classes int32 [n, k];
+ *   1 <= k <= min(num_classes, 32)
+ */
+int edet_softmax_topk(const float* logits, int n, int num_classes, int k, float* probs,
+                      int32_t* classes, edet_stream_t stream);
+
+/*
  * Class-predict 1x1 convolution of ONE pyramid level fused with the class half of pre-NMS: the
  * [n, h, w, num_anchors * num_classes] logits are never written; per pixel and anchor the kernel
  * rounds each logit to fp16 (what edet_pointwise_conv would have stored), takes max / first
