@@ -22,9 +22,10 @@ download, training (dropout, survival_prob / drop_connect are identities at infe
 
 Variable names follow the Keras layer names of the reference: <model>/stem/conv2d/kernel,
 <model>/blocks_<i>/{conv2d, conv2d_1, depthwise_conv2d, se/conv2d, se/conv2d_1,
-tpu_batch_normalization[_n]}, <model>/head/conv2d/kernel; the un-named BN layers of Stem / Head get
-Keras' default 'batch_normalization', the un-named Dense layer 'dense' (<model>/dense/kernel
-[head_filters, num_classes], <model>/dense/bias).
+tpu_batch_normalization[_n]}, <model>/head/conv2d/kernel; the un-named BN layers of Stem / Head are
+named 'tpu_batch_normalization' by the reference's utils.BatchNormalization (utils.py:209-215), the
+un-named Dense layer gets Keras' default 'dense' (<model>/dense/kernel [head_filters, num_classes],
+<model>/dense/bias).
 """
 import collections
 import math
@@ -78,6 +79,7 @@ class EffNetV2Arch(object):
     self.cfg = cfg
     m = self.mconfig = cfg.model
     self.model_name = model_name
+    self.model_config = model_config    # the override as given, for checkers that re-resolve it
     if m.act_fn not in ('silu', 'swish', 'relu6'):
       raise NotImplementedError('act_fn %s' % m.act_fn)
     self.act = utils.ACT_RELU6 if m.act_fn == 'relu6' else utils.ACT_SWISH
@@ -116,7 +118,7 @@ def variable_specs(arch, include_top=False):
   s = collections.OrderedDict()
   mn = arch.model_name
   s['%s/stem/conv2d/kernel' % mn] = VarSpec((3, 3, 3, arch.stem_filters), 'conv', True)
-  _bn(s, '%s/stem/batch_normalization' % mn, arch.stem_filters)
+  _bn(s, '%s/stem/tpu_batch_normalization' % mn, arch.stem_filters)
   for b in arch.blocks:
     sc = '%s/%s' % (mn, b.name)
     if b.expand_name:
@@ -140,7 +142,7 @@ def variable_specs(arch, include_top=False):
     s[last_bn + '/gamma'] = VarSpec((b.output_filters,), 'gamma_res' if b.has_skip else 'gamma', True)
   s['%s/head/conv2d/kernel' % mn] = VarSpec((1, 1, arch.blocks[-1].output_filters, arch.head_filters),
                                             'conv', True)
-  _bn(s, '%s/head/batch_normalization' % mn, arch.head_filters)
+  _bn(s, '%s/head/tpu_batch_normalization' % mn, arch.head_filters)
   if include_top and arch.mconfig.num_classes:
     s['%s/dense/kernel' % mn] = VarSpec((arch.head_filters, arch.mconfig.num_classes), 'dense', True)
     s['%s/dense/bias' % mn] = VarSpec((arch.mconfig.num_classes,), 'dense_bias', True)
@@ -243,7 +245,7 @@ class EffNetV2Model(LaunchList):
 
     # stem: conv3x3 s2 3 -> C + BN + act (Stem :409-432)
     h, wd = -(-h // 2), -(-wd // 2)
-    x = self._stem(w, mn + '/stem/conv2d', mn + '/stem/batch_normalization', (h, wd))
+    x = self._stem(w, mn + '/stem/conv2d', mn + '/stem/tpu_batch_normalization', (h, wd))
     self.endpoints['stem'] = x
     self._se_accumulators(a.blocks)
     red = 0
@@ -285,7 +287,7 @@ class EffNetV2Model(LaunchList):
         red += 1
         self.endpoints['reduction_%d' % red] = y
     self.endpoints['features'] = x
-    hw_, hb_ = conv_w('%s/head/conv2d/kernel' % mn, '%s/head/batch_normalization' % mn)
+    hw_, hb_ = conv_w('%s/head/conv2d/kernel' % mn, '%s/head/tpu_batch_normalization' % mn)
     head = self._buf('head_1x1', (n, h, wd, a.head_filters))
     self._add('head_1x1', lambda x=x, head=head: ops.pointwise_conv(x, hw_[0], hb_, head, act),
               'pointwise_tc', nbytes=2 * (x.numel() + head.numel()),

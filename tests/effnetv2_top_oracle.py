@@ -20,10 +20,10 @@ class EffNetV2TopOracle(effnetv2_oracle.EffNetV2Oracle):
 
   def __call__(self, images):
     ep = super().__call__(images)
-    a, mn = self.arch, self.arch.model_name
+    s, mn = self.s, self.model_name
     pooled = ep['head_1x1'].mean((2, 3))
     ep['pooled_features'] = ep['head'] = (
-        pooled.view(pooled.shape[0], 1, 1, -1) if a.mconfig.local_pooling else pooled)
-    if a.mconfig.num_classes:
+        pooled.view(pooled.shape[0], 1, 1, -1) if s.local_pooling else pooled)
+    if s.num_classes:
       ep['logits'] = pooled @ self.w[mn + '/dense/kernel'] + self.w[mn + '/dense/bias']
     return ep

@@ -82,11 +82,14 @@ def device_weights(arch, w, round_gemm_weights=True):
   return out
 
 
-def effnetv2_device_weights(arch, w):
+def effnetv2_device_weights(arch, w, model_config=None):
   """The same for the EfficientNet V1 / V2 backbone (EffNetV2Model._build, lowering.py): BN
-  folded into fp16 conv kernels (1x1 and k x k), fp32 depthwise taps."""
+  folded into fp16 conv kernels (1x1 and k x k), fp32 depthwise taps.  The layers are the oracle's
+  own (oracle/effnetv2_oracle.py::structure_of), not the product's."""
+  from oracle import effnetv2_oracle  # pylint: disable=g-import-not-at-top
+  st = effnetv2_oracle.structure_of(arch, model_config)
   out = dict(w)
-  mn, eps = arch.model_name, arch.bn_eps
+  mn, eps = st.model_name, st.bn_epsilon
 
   def fold(kernel, bn, depthwise=False):
     g, b = np.float64(w[bn + '/gamma']), np.float64(w[bn + '/beta'])
@@ -99,24 +102,25 @@ def effnetv2_device_weights(arch, w):
     out[bn + '/moving_mean'] = np.zeros_like(g, np.float32)
     out[bn + '/beta'] = (b - m * s).astype(np.float32)
 
-  fold(mn + '/stem/conv2d/kernel', mn + '/stem/batch_normalization')
-  for b in arch.blocks:
-    sc = '%s/%s' % (mn, b.name)
-    if b.expand_name:
-      fold('%s/%s/kernel' % (sc, b.expand_name), '%s/%s' % (sc, b.expand_bn))
-    if b.dw_bn:
-      fold(sc + '/depthwise_conv2d/depthwise_kernel', '%s/%s' % (sc, b.dw_bn), depthwise=True)
-    fold('%s/%s/kernel' % (sc, b.project_name), '%s/%s' % (sc, b.project_bn))
-  fold(mn + '/head/conv2d/kernel', mn + '/head/batch_normalization')
+  fold(mn + '/stem/conv2d/kernel', mn + '/stem/tpu_batch_normalization')
+  for b in st.blocks:
+    sc = '%s/%s' % (mn, b['name'])
+    if b['expand_name']:
+      fold('%s/%s/kernel' % (sc, b['expand_name']), '%s/%s' % (sc, b['expand_bn']))
+    if b['dw_bn']:
+      fold(sc + '/depthwise_conv2d/depthwise_kernel', '%s/%s' % (sc, b['dw_bn']), depthwise=True)
+    fold('%s/%s/kernel' % (sc, b['project_name']), '%s/%s' % (sc, b['project_bn']))
+  fold(mn + '/head/conv2d/kernel', mn + '/head/tpu_batch_normalization')
   return out
 
 
-def effnetv2_format_errors(arch, w, x):
+def effnetv2_format_errors(arch, w, x, model_config=None):
   """{endpoint: rel-L2 of the format model vs the fp32 oracle} and the fp32 endpoints."""
   from oracle import effnetv2_oracle  # pylint: disable=g-import-not-at-top
-  ref = effnetv2_oracle.EffNetV2Oracle(arch, w, torch.float32)(x)
-  mod = effnetv2_oracle.EffNetV2Oracle(arch, effnetv2_device_weights(arch, w), torch.float32,
-                                       store=eo.fp16_store)(x)
+  ref = effnetv2_oracle.EffNetV2Oracle(arch, w, torch.float32, model_config=model_config)(x)
+  mod = effnetv2_oracle.EffNetV2Oracle(arch, effnetv2_device_weights(arch, w, model_config),
+                                       torch.float32, store=eo.fp16_store,
+                                       model_config=model_config)(x)
   return {k: DeviceModel.rel_l2(mod[k], ref[k]) for k in ref}, ref
 
 

@@ -262,6 +262,30 @@ def test_serve_stream_yields_the_logits():
   assert first.is_pinned() and first.numel() * first.element_size() == 2 * 1000 * 4
 
 
+@pytest.mark.parametrize('name,config', [
+    ('efficientnet-b3', None),                                                 # width 1.2, depth 1.4, stem 40
+    ('efficientnetv2-b0', {'width_coefficient': 1.3, 'depth_coefficient': 1.2}),
+    ('efficientnetv2-b0', {'act_fn': 'relu6'})])
+def test_unrun_structures_end_to_end(name, config):
+  """Structures no other test runs through the whole device network, against the oracle's own
+  structure (oracle/effnetv2_structure.py, pinned to the reference constructor): every reduction
+  endpoint, 'head_1x1' and the logits within 1e-3 rel-L2, or within 1.5 x the format model + 1e-4
+  where that is the larger (DESIGN.md section 6)."""
+  import precision_model as pm
+  arch, w, model, x = _build(name, 64, 2, config=config)
+  logits = model(torch.from_numpy(x)).clone()
+  torch.cuda.synchronize()
+  mod, ref = top_format_model(arch, w, x)
+  keys = ['reduction_%d' % i for i in range(1, len(arch.reductions) + 1)] + ['head_1x1', 'logits']
+  assert len(arch.reductions) == 5 and set(keys) <= set(ref)
+  for key in keys:
+    got = logits.cpu() if key == 'logits' else model.endpoints[key].float().cpu().permute(0, 3, 1, 2)
+    merr, err = rel_l2(mod[key], ref[key]), rel_l2(got, ref[key])
+    print('%s %s %s: device %.2e, format model %.2e' % (name, config, key, err, merr))
+    assert err <= max(1e-3, pm.bar(merr)), (key, err, merr)
+  _check_argmax(logits, ref['logits'])
+
+
 @pytest.mark.parametrize('config', [{'num_classes': 0}, {'local_pooling': True},
                                     {'num_classes': 1001, 'headbias': -2.5}])
 def test_config_overrides(config):
