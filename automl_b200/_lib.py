@@ -111,7 +111,8 @@ def load():
   # A/B switches from the environment (scripts/, bench.py runs): EDET_DW_IMPL, EDET_PW_TEAMS
   for env, opt in (('EDET_DW_IMPL', b'dw_impl'), ('EDET_PW_TEAMS', b'pw_teams'),
                    ('EDET_STEM_IMPL', b'stem_impl'), ('EDET_SEPCONV_IMPL', b'sepconv_impl'),
-                   ('EDET_PW_SMEM_KB', b'pw_smem_kb'), ('EDET_PERSIST_SLACK', b'persist_slack')):
+                   ('EDET_PW_SMEM_KB', b'pw_smem_kb'), ('EDET_PERSIST_SLACK', b'persist_slack'),
+                   ('EDET_PW_SHARE_W', b'pw_share_w')):
     if os.environ.get(env):
       if lib.edet_set_option(opt, int(os.environ[env])) != 0:
         raise EdetError('bad %s=%s' % (env, os.environ[env]))

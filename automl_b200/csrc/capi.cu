@@ -29,6 +29,7 @@ static Option g_options[] = {
     {"pw_smem_kb", 0, 227, {0}},     // 0 auto, else shared-memory budget of a pointwise_tc CTA
     {"persist_slack", 0, 132, {0}},  // CTAs a persistent kernel leaves out of its grid
     {"max_ctas", 0, 4096, {0}},      // 0 no cap, else the grid of a persistent kernel (at most its work)
+    {"pw_share_w", 0, 1, {0}},       // 0 auto, 1 = pointwise_tc streams W per 64-row tile
 };
 static Option* find_option(const char* name) {
   for (Option& o : g_options)
@@ -43,6 +44,7 @@ int option_pw_teams() { return option_value(3); }
 int option_pw_smem_kb() { return option_value(4); }
 int option_persist_slack() { return option_value(5); }
 int option_max_ctas() { return option_value(6); }
+int option_pw_share_w() { return option_value(7); }
 
 int current_device() {
   int dev = -1;

@@ -190,6 +190,7 @@ int option_pw_teams();  // 0 auto, 2 / 3 = force that many epilogue teams in poi
 int option_pw_smem_kb();     // 0 auto, else the shared-memory budget (KiB) of a pointwise_tc CTA
 int option_persist_slack();  // CTAs a persistent kernel leaves out of its grid (default 0)
 int option_max_ctas();       // 0 (default): no cap, else the exact grid of a persistent kernel
+int option_pw_share_w();     // 0 auto, 1 = pointwise_tc keeps 64-row tiles where W streams
 constexpr int kMaxDevices = 64;
 int current_device();                 // ordinal of the current device, -1 (+ error text) on failure
 int device_sm_count();                // multiprocessor count of the current device, 0 on failure

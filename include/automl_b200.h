@@ -66,6 +66,12 @@ const char* edet_last_error(void);
  * 162 KiB up with two consumers and from 226 KiB with three (the widest plan: 128 x 64 W tiles
  * streamed with A, nout 8192); a smaller budget refuses the shapes it cannot hold with
  * EDET_ERR_INVALID;
+ * "pw_share_w" = 0 (default: where W streams with A -- per-image SE weights, or shared weights too
+ * large to stay in shared memory --, the launch has at least one 128-row tile per CTA and, with a
+ * residual, K spans at least 10 k-blocks of 64, both
+ * consumers of a CTA compute one 128-row tile, 64 rows each, against one W tile per k-block; with
+ * three consumers or a pw_smem_kb budget that cannot hold four such stages, 64-row tiles) | 1 (64-row
+ * tiles, each with its own W tile, as with three consumers);
  * "persist_slack" = CTAs a persistent kernel leaves out of its grid (default 0);
  * "max_ctas" = 0 (default: no cap) | 1..4096: the most CTAs a persistent kernel launches.
  * Every persistent kernel (pointwise / class arg-max, tiled depthwise, conv2d, conv2d_transpose,
