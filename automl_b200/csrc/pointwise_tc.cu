@@ -115,7 +115,9 @@ constexpr int kArgmaxCols = 96;   // columns per anchor in the padded class-head
 struct TileCoord {
   int b, m_blk, n_blk;
 };
-constexpr int kMaxBiasSmem = 8192;
+// Bias floats staged in shared memory: whole 128-column N tiles of the widest registered layer,
+// the 8256-channel expand of efficientnet-l2 (65 tiles).  Narrower launches stage only their own.
+constexpr int kMaxBiasSmem = 65 * kMaxBlockN;
 
 // Work unit u -> batch entry, first M block, N tile (the first one when the unit holds A).
 __device__ __forceinline__ TileCoord decode_unit(int u, const Params& p) {

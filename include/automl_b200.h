@@ -63,8 +63,8 @@ const char* edet_last_error(void);
  * "sepconv_impl" = 0 (default: TMA-staged input tile for c <= 64, one buffer, four CTAs per SM) |
  * 1 (loads from global) | 2 (TMA, two buffers, three CTAs per SM);
  * "pw_smem_kb" = 0 (default: 227 KiB, one pointwise CTA per SM) | 64..227: every shape runs from
- * 162 KiB up with two consumers and from 226 KiB with three (the widest plan: 128 x 64 W tiles
- * streamed with A, nout 8192); a smaller budget refuses the shapes it cannot hold with
+ * 163 KiB up with two consumers and from 227 KiB with three (the widest plan: 128 x 64 W tiles
+ * streamed with A, nout 8256 up to 8320); a smaller budget refuses the shapes it cannot hold with
  * EDET_ERR_INVALID;
  * "pw_share_w" = 0 (default: where W streams with A -- per-image SE weights, or shared weights too
  * large to stay in shared memory --, the launch has at least one 128-row tile per CTA and, with a

@@ -17,8 +17,9 @@ DEV = 'cuda:0'
 COLS = 96   # ops.CLASS_ARGMAX_COLS
 SCORE_SENTINEL, CLASS_SENTINEL = -5.0, -7
 
-# Every k here is a multiple of 16, so the last k-step ends at k and the A columns past k never
-# enter an MMA: the lda > k cases check the row pitch of the A map, not a K tail.  K-tail leakage
+# Every k here but lite3x's 200 is a multiple of 16, so the last k-step ends at k and the A columns
+# past k never enter an MMA: the lda > k cases check the row pitch of the A map, not a K tail.  K 200
+# ends in an 8-wide k16 step, whose other 8 columns are TMA zero fill (lda == k).  K-tail leakage
 # (NaN past k in A) is tested on the A map the two paths share, in
 # test_gpu_pointwise_plans.test_pointwise_strided_operands.  The arg-max kernel always has two
 # consumers, so the pw_teams=3 setting runs the default plan.
@@ -32,6 +33,7 @@ CASES = [
     (3, 20, 112, 128, 1, 33, 31, 123, 7),      # ragged rows, lda > k, resident W, 2 k-blocks
     (1, 1, 160, 168, 1, 17, 19, 5, 3),         # one class of one anchor, lda > k
     (3, 20, 160, 160, 3, 20, 21, 0, 11),       # D3 head width, resident W over 3 k-blocks
+    (9, 90, 200, 200, 2, 13, 11, 40, 5),       # lite3x head width: streamed W, K tail of 8
     (9, 90, 224, 224, 1, 12, 12, 0, 0),        # D4 head width, streamed W
     (9, 90, 288, 296, 3, 9, 9, 11, 2),         # D5/D6 head width, streamed W, lda > k
     (9, 90, 384, 384, 1, 5, 5, 81, 0),         # D7 head width, streamed W

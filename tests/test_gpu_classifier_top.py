@@ -271,6 +271,10 @@ def test_unrun_structures_end_to_end(name, config):
   structure (oracle/effnetv2_structure.py, pinned to the reference constructor): every reduction
   endpoint, 'head_1x1' and the logits within 1e-3 rel-L2, or within 1.5 x the format model + 1e-4
   where that is the larger (DESIGN.md section 6)."""
+  _check_end_to_end(name, config)
+
+
+def _check_end_to_end(name, config):
   import precision_model as pm
   arch, w, model, x = _build(name, 64, 2, config=config)
   logits = model(torch.from_numpy(x)).clone()
@@ -284,6 +288,16 @@ def test_unrun_structures_end_to_end(name, config):
     print('%s %s %s: device %.2e, format model %.2e' % (name, config, key, err, merr))
     assert err <= max(1e-3, pm.bar(merr)), (key, err, merr)
   _check_argmax(logits, ref['logits'])
+
+
+def test_efficientnet_l2_end_to_end():
+  """efficientnet-l2 at 64 x 64, batch 2, include_top=True, as test_unrun_structures_end_to_end
+  checks the others.  Its blocks 83-87 expand 1376 to 8256 channels, the widest 1x1 convolution
+  of any registered model (65 N tiles of 128 columns), which pointwise_tc once refused as too wide
+  for its shared-memory bias.  481 M parameters: the synthetic weights alone are 1.9 GB of float32
+  on the host.  On an H100 80GB HBM3 host the test took 31 s (weights, upload, the device pass and
+  two CPU oracle passes) and its process peaked at 8.6 GB of resident host memory."""
+  _check_end_to_end('efficientnet-l2', None)
 
 
 @pytest.mark.parametrize('config', [{'num_classes': 0}, {'local_pooling': True},

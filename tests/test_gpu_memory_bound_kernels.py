@@ -24,7 +24,8 @@ from automl_b200._lib import EdetError
 from automl_b200.efficientnetv2 import effnetv2_model
 from oracle import efficientdet_oracle as eo
 from test_gpu_persistent_kernels import (  # noqa: F401  (the shared harness)
-    DEV, GUARD, SENTINEL, V2_MODELS, Out, _kernel_grids, carve, check_close, over_grids, span_bias)
+    DEV, GUARD, SENTINEL, V1_MODELS, V2_MODELS, Out, _kernel_grids, carve, check_close, over_grids,
+    span_bias)
 
 NONE, SWISH, RELU6 = utils.ACT_NONE, utils.ACT_SWISH, utils.ACT_RELU6
 U = 2.0**-24                  # fp32 unit roundoff
@@ -85,12 +86,12 @@ def _equal(a, b):
 
 # ---------------------------------------------------------------------------------------------
 # shape registries (no GPU)
-def dw_shapes():
+def dw_shapes(classifiers=V1_MODELS + V2_MODELS):
   """(k, stride, c, has_se, act) of every depthwise convolution of the registered models: the
   MBConv blocks of EfficientDet D0-D7x and lite0-lite4 (relu6, no SE), the MBConv (conv_type 0)
-  blocks of the EfficientNetV2 models, and the bias-free 3x3 depthwise of the head / predict layers
-  (ACT_NONE) at every feature-network width.  Every block depthwise has a bias, the head ones
-  none."""
+  blocks of the EfficientNet V1 and V2 classifiers (or those named), and the bias-free 3x3
+  depthwise of the head / predict layers (ACT_NONE) at every feature-network width.  Every block
+  depthwise has a bias, the head ones none."""
   shapes = set()
   for name in DET_MODELS:
     a = _det_arch(name)
@@ -98,7 +99,7 @@ def dw_shapes():
     for b in a.blocks:
       shapes.add((b.kernel_size, b.stride, b.mid_filters, bool(b.se_filters), act))
     shapes.add((3, 1, a.fpn_filters, False, NONE))
-  for name in V2_MODELS:
+  for name in classifiers:
     v = effnetv2_model.EffNetV2Arch(name)
     for b in v.blocks:
       if b.conv_type == 0:
@@ -106,14 +107,14 @@ def dw_shapes():
   return sorted(shapes)
 
 
-def se_shapes():
+def se_shapes(classifiers=V1_MODELS + V2_MODELS):
   """(c = mid_filters, se, nout = output_filters) of every SE block of the same models."""
   shapes = set()
   for name in DET_MODELS:
     for b in _det_arch(name).blocks:
       if b.se_filters:
         shapes.add((b.mid_filters, b.se_filters, b.output_filters))
-  for name in V2_MODELS:
+  for name in classifiers:
     for b in effnetv2_model.EffNetV2Arch(name).blocks:
       if b.conv_type == 0 and b.se_filters:
         shapes.add((b.mid_filters, b.se_filters, b.output_filters))
@@ -133,6 +134,14 @@ def _node_signature(a, node):
       modes.append((r.mode, r.pool))
       hws.append(r.in_hw)
   return tuple(modes), tuple(hws)
+
+
+def _stable_order(registry):
+  """The shapes of registry(): those of the detectors and the V2 classifiers first, in their own
+  sorted order, then the ones only the V1 classifiers add.  A case's map and batch follow its
+  index, so the cases of the earlier shapes stay what they were when the V1 shapes joined."""
+  base = registry(V2_MODELS)
+  return base + [shape for shape in registry() if shape not in base]
 
 
 def _pools(a):
@@ -218,7 +227,7 @@ def _reg_map(h, w, c, s):
 
 def _dw_cases():
   cases = []
-  for i, (k, s, c, se, act) in enumerate(dw_shapes()):
+  for i, (k, s, c, se, act) in enumerate(_stable_order(dw_shapes)):
     n = 2 if c <= 512 else 1
     th, tw = TILED_MAPS[(k, s)][i % 2]
     rh, rw = _reg_map(*REG_MAPS[(k, s)][i % 2], c, s)
@@ -503,7 +512,7 @@ def _se_cases():
   every split; swish as in the registered models, relu6 on every fifth shape (se_fc1 applies the
   block's activation)."""
   cases = []
-  for i, (c, se, nout) in enumerate(se_shapes()):
+  for i, (c, se, nout) in enumerate(_stable_order(se_shapes)):
     n = (1, 2, 3, 5)[i % 4] if nout * c < 10**6 else (1, 2)[i % 2]
     cases.append((n, c, se, nout, RELU6 if i % 5 == 4 else SWISH))
   return cases
@@ -770,6 +779,8 @@ def test_dw_registry_shapes_are_covered():
   assert any(128 % (c // 2) and c // 2 < 128 for _, _, c, _, _ in shapes)
   assert {(k, s) for k, s, _, _, _ in shapes} == set(DW_TILE)
   assert {F for k, s, F, se, act in shapes if act == NONE} == {64, 88, 112, 160, 200, 224, 288, 384}
+  # the V1 classifiers' widest maps (efficientnet-l2, -b8)
+  assert {(3, 1, 8256, True, SWISH), (5, 1, 4944, True, SWISH), (5, 2, 2880, True, SWISH)} <= set(shapes)
   covered = {}
   for n, h, w, c, k, s, act, b, se in DW_CASES:
     assert b == (act != NONE) or (act, b, se) in DW_COMBOS
@@ -788,7 +799,8 @@ def test_dw_registry_shapes_are_covered():
 
 def test_se_registry_shapes_are_covered():
   shapes = se_shapes()
-  assert min(se for _, se, _ in shapes) == 4 and max(se for _, se, _ in shapes) == 160
+  assert min(se for _, se, _ in shapes) == 4 and max(se for _, se, _ in shapes) == 344
+  assert (8256, 344, 1376) in shapes                   # efficientnet-l2 blocks 83-87
   assert any(se % 4 for _, se, _ in shapes)            # se_fc2's tail loop
   assert {(c, se, nout) for _, c, se, nout, _ in SE_CASES} == set(shapes)
   assert {se_split(n, c, se) for n, c, se, _, _ in SE_CASES} == {1, 2, 4, 8}

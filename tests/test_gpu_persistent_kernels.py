@@ -38,6 +38,7 @@ FLOOR = 5e-5
 NONE, SWISH, RELU6 = utils.ACT_NONE, utils.ACT_SWISH, utils.ACT_RELU6
 ACTS = (SWISH, RELU6, NONE)  # what conv2d, sepconv and the stem accept
 V2_MODELS = ['efficientnetv2-%s' % v for v in ('b0', 'b1', 'b2', 'b3', 's', 'm', 'l', 'xl')]
+V1_MODELS = ['efficientnet-b%d' % i for i in range(9)] + ['efficientnet-l2']
 
 
 def _ops():
@@ -321,6 +322,11 @@ def _stem_cases():
   for i, cout in enumerate(range(8, 65, 8)):
     for d, dist in enumerate(('normal', 'wide')):
       cases.append(images[(i + 3 * d) % 6] + (cout, dist, ACTS[(i + d) % 3]))
+  # the stems of efficientnet-b8 and -l2, wider than the tensor-core stem takes: under the default
+  # stem_impl they run on the CUDA-core kernel, in 64-channel slabs (the last one partly live)
+  for i, cout in enumerate((72, 136)):
+    for d, dist in enumerate(('normal', 'wide')):
+      cases.append(images[(2 * i + 3 * d + 1) % 6] + (cout, dist, ACTS[(i + 2 * d) % 3]))
   return cases
 
 
