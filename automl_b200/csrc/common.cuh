@@ -213,11 +213,19 @@ inline int ensure_dynamic_smem(F kernel, int bytes, int* done) {
 }
 
 // Programmatic dependent launch (PDL): every kernel of the path is launched with the
-// programmatic-stream-serialization attribute, signals `launch_dependents` as its first
-// instruction and executes `griddepcontrol.wait` before it touches global memory.  The NEXT
-// kernel's CTAs may therefore be scheduled, and run their prologue (smem carve-up, mbarrier
-// init, descriptor prefetch, weight preload into registers is NOT done before
-// the wait), while the tail of the previous kernel drains -- the step is ~220 short launches.
+// programmatic-stream-serialization attribute and signals `launch_dependents` as its first
+// instruction, so the NEXT kernel's CTAs may be scheduled and run their prologue while the tail of
+// the previous kernel drains -- the step is ~220 short launches.  Before its own `pdl_wait_prior()`
+// a kernel may only
+//  - set up shared memory and mbarriers and prefetch tensor-map descriptors;
+//  - read CONSTANTS: buffers the host wrote before the first launch and no kernel ever writes
+//    (weights, biases, depthwise taps, fusion weights), into registers or shared memory.
+// It must not read anything a kernel writes (activations, SE sums, SE-scaled or per-image weights:
+// the previous kernel may still be writing them) and must not write global memory at all (the
+// previous kernel may still be reading it).  The wait returns only when every prior grid has
+// completed and flushed, so after it both are safe.  DESIGN.md section 4 lists each family's
+// pre-wait reads; a caller must never pass a device-computed buffer as one of them.
+// tests/test_gpu_pdl_chains.py and tests/test_pdl_sass.py check this rule.
 __device__ __forceinline__ void pdl_launch_dependents() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
