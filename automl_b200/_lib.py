@@ -37,6 +37,8 @@ SIGNATURES = {
     'edet_preprocess': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                 ctypes.POINTER(c_float), ctypes.POINTER(c_float),
                                 ctypes.POINTER(c_float), c_void_p]),
+    'edet_preprocess_ragged': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                       ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p]),
     'edet_stem_conv': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                c_int, c_int, c_void_p]),
     'edet_pointwise_conv': (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int,

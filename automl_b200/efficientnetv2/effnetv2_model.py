@@ -38,7 +38,7 @@ from automl_b200 import utils
 from automl_b200.backbone.efficientnet_builder import _layer_namer
 from automl_b200.efficientnetv2 import effnetv2_configs
 from automl_b200.efficientnetv2 import preprocessing
-from automl_b200.lowering import LaunchList, bn_fold
+from automl_b200.lowering import LaunchList, bn_fold, capture_graph
 from automl_b200.weights import VarSpec, _bn
 
 Block = collections.namedtuple('Block', [
@@ -326,10 +326,7 @@ class EffNetV2Model(LaunchList):
       if self._graph is None:
         self._run_ops()                      # warm-up (loads kernels, sets attributes)
         torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-          self._run_ops()
-        self._graph = g
+        self._graph = capture_graph(self._run_ops)
       self._graph.replay()
 
   def __call__(self, images=None, training=False, with_endpoints=False):

@@ -22,7 +22,7 @@ from automl_b200 import anchors as anchors_lib
 from automl_b200 import ops
 from automl_b200 import utils
 from automl_b200.arch import DetArch
-from automl_b200.lowering import LaunchList, bn_fold
+from automl_b200.lowering import LaunchList, bn_fold, capture_graph
 
 
 def _round_up(x, m):
@@ -573,10 +573,7 @@ class Engine(LaunchList):
       if warm:
         fn()                                 # warm-up outside capture (kernel attributes, modules)
       torch.cuda.synchronize(self.device)
-      g = torch.cuda.CUDAGraph()
-      with torch.cuda.graph(g, stream=capture_stream):
-        fn()
-      self._graph[key] = g
+      self._graph[key] = capture_graph(fn, capture_stream)
     return self._graph[key]
 
   def run(self, postprocess=True, after_nms=None):

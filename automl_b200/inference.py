@@ -18,8 +18,9 @@ TensorRT — SURVEY.md section 2 row 8).
 gives seeded synthetic weights; a path to an .npz whose keys are the reference variable names
 (Keras layouts, see weights.py) loads real weights.
 
-The whole request runs on the device: H2D copy of the uint8 images -> edet_preprocess ->
-network -> pre-NMS -> NMS -> D2H copy of the [N, max_output_size, 7] detections.
+The whole request runs on the device: H2D copy of the uint8 images -> edet_preprocess (images of
+one size) or edet_preprocess_ragged (sizes differ; one launch either way) -> network -> pre-NMS ->
+NMS -> D2H copy of the [N, max_output_size, 7] detections.
 """
 import copy
 import io
@@ -89,6 +90,44 @@ def image_preprocess(image, image_size, mean_rgb, stddev_rgb, device='cuda:0'):
   out = torch.empty(1, oh, ow, 3, dtype=torch.float32, device=device)
   scale = ops.preprocess(raw, out, _rgb3(mean_rgb), _rgb3(stddev_rgb))
   return out[0], scale
+
+
+def preprocess_table(shapes, image_size):
+  """The table of a ragged pre-process (ops.preprocess_ragged) for images of sizes `shapes`
+  [(h, w), ...], packed in this order, each at a 16-byte aligned offset: (int32 [N, 6]
+  edet_preprocess_image rows, packed byte count, float32 [N] image_scale_to_original).
+
+  Scale-to-fit in float32 as edet_preprocess computes it (dataloader.py:115-127, inference.py:68-109
+  runs image_preprocess per image): s = min(H / h, W / w), scaled = int(h * s), w likewise, and
+  1 / s.  Raises ValueError for an empty image or one whose scaled size is 0."""
+  from automl_b200 import utils
+  oh, ow = utils.parse_image_size(image_size)
+  hw = np.asarray(shapes, np.int64).reshape(-1, 2)
+  if len(hw) == 0 or (hw < 1).any():
+    raise ValueError('empty image or request: sizes %s' % hw.tolist())
+  h, w = hw[:, 0].astype(np.float32), hw[:, 1].astype(np.float32)
+  sy, sx = np.float32(oh) / h, np.float32(ow) / w
+  scale = np.where(sx < sy, sx, sy)
+  scaled_h, scaled_w = (h * scale).astype(np.int64), (w * scale).astype(np.int64)
+  bad = np.flatnonzero((scaled_h < 1) | (scaled_w < 1))
+  if len(bad):
+    i = bad[0]
+    raise ValueError('a %dx%d image collapses to %dx%d at %dx%d'
+                     % (hw[i, 0], hw[i, 1], scaled_h[i], scaled_w[i], oh, ow))
+  nbytes = 3 * hw[:, 0] * hw[:, 1]
+  offsets = np.zeros(len(hw), np.int64)
+  offsets[1:] = np.cumsum((nbytes[:-1] + 15) // 16 * 16)
+  desc = np.zeros((len(hw), ops.PRE_DESC_WORDS), np.int32)
+  desc[:, :2] = offsets.view(np.int32).reshape(-1, 2)
+  desc[:, 2:] = np.stack([hw[:, 0], hw[:, 1], scaled_h, scaled_w], axis=1)
+  return desc, int(offsets[-1] + nbytes[-1]), np.float32(1.0) / scale
+
+
+def _grow(buf, nbytes, **kw):
+  """`buf` if it holds `nbytes`, else a new uint8 buffer of at least twice its size."""
+  if buf is not None and buf.numel() >= nbytes:
+    return buf
+  return torch.empty(max(nbytes, 2 * buf.numel() if buf is not None else 0), dtype=torch.uint8, **kw)
 
 
 def _rgb3(v):
@@ -194,7 +233,7 @@ class ServingDriver(object):
           'scales': torch.empty(n, dtype=torch.float32).pin_memory(),
           'gathered': (torch.empty(world * n, eng.max_output_size, 7, device=self.device)
                        if world > 1 else None),
-          'raw_host': None, 'raw_dev': None,
+          'raw_host': None, 'raw_dev': None, 'packed_host': None, 'packed_dev': None,
           'ev_h2d': torch.cuda.Event(), 'ev_raw_free': torch.cuda.Event(),
           'ev_done': torch.cuda.Event(), 'pending': None,
       } for _ in range(self.MAX_IN_FLIGHT)]
@@ -203,7 +242,9 @@ class ServingDriver(object):
   # ---- serving -------------------------------------------------------------------------------
   def _stage_raw(self, eng, slot, image_arrays):
     """Uploads the uint8 images (copy stream, from pinned memory) and runs the device pre-process
-    into the engine input (current stream)."""
+    into the engine input (current stream): images of one size as one [N, h, w, 3] batch, images
+    of different sizes packed behind a descriptor table (preprocess_table), checked before anything
+    is enqueued: an image that is not uint8 [h, w, 3] or collapses to zero size raises ValueError."""
     n = eng.n
     main = torch.cuda.current_stream()
     if isinstance(image_arrays, torch.Tensor):   # [N,h,w,3] uint8 (e.g. pinned host memory)
@@ -237,10 +278,33 @@ class ServingDriver(object):
       scale = ops.preprocess(slot['raw_dev'], eng.input, self.mean_rgb, self.stddev_rgb)
       slot['ev_raw_free'].record(main)
       slot['scales'].fill_(scale)
-    else:  # ragged batch: one pre-process launch per image (like the reference's python loop)
-      for i, im in enumerate(image_arrays):
-        raw = torch.as_tensor(np.ascontiguousarray(im), dtype=torch.uint8).to(self.device)[None]
-        slot['scales'][i] = ops.preprocess(raw, eng.input[i:i + 1], self.mean_rgb, self.stddev_rgb)
+    else:  # ragged batch: descriptor rows, then the packed images; one H2D, one launch
+      images = [np.asarray(im) for im in image_arrays]
+      for im in images:
+        if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+          raise ValueError('expected uint8 [h, w, 3] images, got %s %s' % (im.dtype, im.shape))
+      desc, total, scales = preprocess_table([im.shape[:2] for im in images],
+                                             tuple(eng.input.shape[1:3]))
+      head = (desc.nbytes + 15) // 16 * 16
+      staged = head + total
+      slot['ev_h2d'].synchronize()          # the slot's previous H2D has read the staging buffer
+      slot['packed_host'] = _grow(slot['packed_host'], staged, pin_memory=True)
+      if slot['packed_dev'] is None or slot['packed_dev'].numel() < staged:
+        main.synchronize()                  # no queued pre-process still reads the old buffer
+        slot['packed_dev'] = _grow(slot['packed_dev'], staged, device=self.device)
+      host, dev = slot['packed_host'].numpy(), slot['packed_dev']
+      host[:desc.nbytes] = desc.view(np.uint8).ravel()
+      for im, off in zip(images, desc[:, :2].copy().view(np.int64)[:, 0]):
+        host[head + off:head + off + im.size] = np.ascontiguousarray(im).reshape(-1)
+      with torch.cuda.stream(self._copy_stream):
+        self._copy_stream.wait_event(slot['ev_raw_free'])   # pre-process of the request before last
+        dev[:staged].copy_(slot['packed_host'][:staged], non_blocking=True)
+        slot['ev_h2d'].record(self._copy_stream)
+      main.wait_event(slot['ev_h2d'])
+      ops.preprocess_ragged(dev[head:staged], dev[:desc.nbytes].view(torch.int32).view(desc.shape),
+                            eng.input, self.mean_rgb, self.stddev_rgb)
+      slot['ev_raw_free'].record(main)
+      slot['scales'].numpy()[:] = scales
     eng.image_scales.copy_(slot['scales'], non_blocking=True)
 
   def submit(self, image_arrays):

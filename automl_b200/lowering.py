@@ -1,11 +1,33 @@
 """What the detector (engine.Engine) and the EfficientNet V1 / V2 classifier
 (efficientnetv2/effnetv2_model.EffNetV2Model) lower the same way: the BatchNorm fold, the recorded
-launch list with its per-launch accounting, and the EfficientNet stem and MBConv blocks."""
+launch list with its per-launch accounting, its capture into a CUDA graph, and the EfficientNet
+stem and MBConv blocks."""
+import gc
+
 import numpy as np
 import torch
 
 from automl_b200 import ops
 from automl_b200 import utils
+
+
+def capture_graph(fn, stream=None):
+  """fn() captured into a new torch.cuda.CUDAGraph (on `stream`, else a side stream torch picks).
+
+  Python's cyclic garbage collector is paused for the capture.  A dropped Engine or model lives in
+  reference cycles until the collector frees it; freed during a capture, its CUDA graphs and pinned
+  buffers are destroyed with CUDA calls that a global-mode capture forbids, and the capture fails at
+  capture_end.  Paused, the collector frees them once the capture has ended."""
+  g = torch.cuda.CUDAGraph()
+  enabled = gc.isenabled()
+  gc.disable()
+  try:
+    with torch.cuda.graph(g, stream=stream):
+      fn()
+  finally:
+    if enabled:
+      gc.enable()
+  return g
 
 
 def bn_fold(w, scope, eps):

@@ -70,6 +70,24 @@ def preprocess(raw, out, mean_rgb, stddev_rgb):
   return scale.value
 
 
+PRE_DESC_WORDS = 6      # int32 words of one edet_preprocess_image row: offset (2 words), h, w, scaled_h, scaled_w
+
+
+def preprocess_ragged(packed, desc, out, mean_rgb, stddev_rgb):
+  """A ragged request in one launch: packed uint8 (the images back to back, HWC), desc int32
+  [N, 6] edet_preprocess_image rows (byte offset into `packed`, h, w, scaled_h, scaled_w; the
+  caller keeps every image inside `packed`) -> out fp32 [N,H,W,3], each image as `preprocess`
+  computes it alone."""
+  n, oh, ow = out.shape[0], out.shape[1], out.shape[2]
+  if tuple(out.shape) != (n, oh, ow, 3) or tuple(desc.shape) != (n, PRE_DESC_WORDS):
+    raise ValueError('preprocess_ragged: out %s must be [N, H, W, 3] and desc %s [N, %d]'
+                     % (tuple(out.shape), tuple(desc.shape), PRE_DESC_WORDS))
+  mean = (ctypes.c_float * 3)(*[float(v) for v in mean_rgb])
+  std = (ctypes.c_float * 3)(*[float(v) for v in stddev_rgb])
+  _lib.call('edet_preprocess_ragged', _ptr(packed, torch.uint8), _ptr(desc, torch.int32),
+            _ptr(out, torch.float32), n, oh, ow, mean, std, _stream())
+
+
 def stem_conv(images, out, w, bias, act):
   """images fp32 [N,H,W,3] -> out fp16 [N,ceil(H/2),ceil(W/2),C]."""
   n, h, wd, c3 = images.shape

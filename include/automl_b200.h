@@ -116,6 +116,27 @@ int edet_preprocess(const uint8_t* in, float* out, int n, int h, int w, int out_
                     edet_stream_t stream);
 
 /*
+ * Serving pre-process of a ragged request (images of different sizes) in one launch: per image the
+ * arithmetic of edet_preprocess, so every output equals edet_preprocess of that image alone, bit
+ * for bit.  Replaces inference.batch_image_preprocess inference.py:68-109 (image_preprocess per
+ * image) and dataloader.DetectionInputProcessor dataloader.py:59-65, 115-142.
+ *   packed  uint8, the images back to back (HWC, 3 channels)
+ *   desc    DEVICE edet_preprocess_image [n]: byte offset of the image in `packed`, its h and w,
+ *           and its scaled size, computed on the host as edet_preprocess does (float32:
+ *           s = min(out_h / h, out_w / w), scaled_h = (int)(h * s), scaled_w = (int)(w * s); the
+ *           image_scale_to_original is 1 / s); every field positive, scaled_h <= out_h, scaled_w <= out_w
+ *   out     float32 [n, out_h, out_w, 3]
+ *   h_mean_rgb / h_stddev_rgb: HOST float32[3]
+ */
+typedef struct {
+  int64_t offset;
+  int32_t h, w, scaled_h, scaled_w;
+} edet_preprocess_image;
+int edet_preprocess_ragged(const uint8_t* packed, const edet_preprocess_image* desc, float* out,
+                           int n, int out_h, int out_w, const float* h_mean_rgb,
+                           const float* h_stddev_rgb, edet_stream_t stream);
+
+/*
  * Stem: Conv2D 3x3 stride 2 'same' (3 -> cout, no bias) + BN + act.
  * Replaces backbone/efficientnet_model.py:511-527 (Stem.call).
  *   in   float32 [n, h, w, 3] NHWC            out  half [n, ceil(h/2), ceil(w/2), cout]
