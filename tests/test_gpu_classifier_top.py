@@ -74,6 +74,15 @@ def _pool(x):
   return out.result()
 
 
+def check_pool(got, x):
+  """got [N, C] within the bound of the fp32 mean of x [N, h, w, C] over its pixels."""
+  n, h, w, c = x.shape
+  x64 = x.double().view(n, h * w, c)
+  ref, mean_abs = x64.mean(1), x64.abs().mean(1)
+  bound = (-(-h * w // 64) + 7) * U * mean_abs * 1.01
+  assert bool(((got.double() - ref).abs() <= bound).all()), float(((got.double() - ref).abs() / bound.clamp_min(1e-30)).max())
+
+
 @pytest.mark.parametrize('c', HEAD_WIDTHS)
 @pytest.mark.parametrize('hw', [(1, 1), (7, 7), (10, 10), (12, 12), (19, 19), (7, 12)])
 def test_global_avg_pool(hw, c):
@@ -81,10 +90,7 @@ def test_global_avg_pool(hw, c):
   n = 128
   x = _randn((n, h, w, c), 1000 * h * w + c, torch.float16, 2.0) + 0.5   # a mean that is not ~0
   got = _pool(x)
-  x64 = x.double().view(n, h * w, c)
-  ref, mean_abs = x64.mean(1), x64.abs().mean(1)
-  bound = (-(-h * w // 64) + 7) * U * mean_abs * 1.01
-  assert bool(((got.double() - ref).abs() <= bound).all()), float(((got.double() - ref).abs() / bound.clamp_min(1e-30)).max())
+  check_pool(got, x)
   assert torch.equal(_pool(x), got)                                # two launches, same bits
   assert torch.equal(_pool(x[:3].contiguous()), got[:3])           # rows do not depend on N
   for i in (0, 77, 127):

@@ -395,6 +395,16 @@ def _mbf_reference(x, we, be, taps, bd, act, k, s):
   return y, zd, m, depthwise_f64(_ulp16(e), taps.abs(), k, s)
 
 
+def check_mbf(got, y, z, m, flip, act, k, what):
+  """The output bound of test_mbconv_expand_dw, from _mbf_reference's (y, z, m, flip)."""
+  dz = flip + (k * k + 1) * U * m
+  tol = _ulp16(y) + FLOOR + _act_slope(z, act, dz) * dz
+  err = (got.double() - y).abs()
+  bad = ~(err <= tol)
+  assert not bool(bad.any()), '%s: max err %g, %d outside the bound, first at %s' % (
+      what, float(err.max()), int(bad.sum()), tuple(bad.nonzero()[0].tolist()))
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize('case', MBF2_CASES, ids=_mbf_id)
 def test_mbconv_expand_dw(case):
@@ -430,12 +440,7 @@ def test_mbconv_expand_dw(case):
   got = res[0] if has_se else res
   assert torch.equal(got, first[0] if has_se else first), 'output depends on the SE start'
   y, z, m, flip = _mbf_reference(x, we, be, taps, bd, act, k, s)
-  dz = flip + (k * k + 1) * U * m
-  tol = _ulp16(y) + FLOOR + _act_slope(z, act, dz) * dz
-  err = (got.double() - y).abs()
-  bad = ~(err <= tol)
-  assert not bool(bad.any()), '%s: max err %g, %d outside the bound, first at %s' % (
-      _mbf_id(case), float(err.max()), int(bad.sum()), tuple(bad.nonzero()[0].tolist()))
+  check_mbf(got, y, z, m, flip, act, k, _mbf_id(case))
   if has_se:
     sums = first[1]
     _check_se_sums(sums, y, z, m + flip / ((k * k + 1) * U), act, k, mbf_partials(h, w, k, s),

@@ -697,12 +697,6 @@ def test_fuse_dw(case):
   devs = [carve_inf(t) if m == 'down' else carve(t) for t, (m, _) in zip(tens, modes)]
   dtaps, dch = carve(taps), carve(torch.from_numpy(channel))
   specs = [(d, code[m], pool, float(wt)) for d, (m, pool), wt in zip(devs, modes, scalar)]
-  res = []     # resampled inputs, NHWC float64 (nearest and max select fp16 values: exact in fp32)
-  for t, (m, pool) in zip(tens, modes):
-    x = t.float().permute(0, 3, 1, 2)
-    x = (x if m == 'same' else eo.resize_nearest_tf1(x, h, w) if m == 'up'
-         else eo.max_pool_same(x, pool[:2], pool[2:]))
-    res.append(x.permute(0, 2, 3, 1).double())
   for per_channel in (False, True):
     def launch():
       out = Out((n, h, w, f))
@@ -710,13 +704,28 @@ def test_fuse_dw(case):
       return out.result()
     got = launch()
     assert torch.equal(launch(), got), 'two runs differ'
-    if per_channel:
-      fused = sum(r * torch.from_numpy(cw.astype(np.float64)) for r, cw in zip(res, channel))
-    else:
-      fused = sum(r * float(wt) for r, wt in zip(res, scalar))
-    fused = {SWISH: lambda t: t * torch.sigmoid(t), RELU6: lambda t: t.clamp(0, 6),
-             NONE: lambda t: t}[act](fused)
-    check_close(got, depthwise_f64(fused, taps, 3, 1), '%s channel=%d' % (_fuse_id(case), per_channel))
+    ref = fuse_reference(tens, modes, (h, w), taps, channel if per_channel else scalar, per_channel, act)
+    check_close(got, ref, '%s channel=%d' % (_fuse_id(case), per_channel))
+
+
+def fuse_reference(tens, modes, hw, taps, weights, per_channel, act):
+  """float64 NHWC resample -> weighted sum (scalar weights, or [inputs, C] per-channel ones) ->
+  activation -> depthwise 3 x 3 of fp16 inputs [N,h,w,F] (nearest and max select fp16 values:
+  exact in fp32)."""
+  h, w = hw
+  res = []
+  for t, (m, pool) in zip(tens, modes):
+    x = t.float().permute(0, 3, 1, 2)
+    x = (x if m == 'same' else eo.resize_nearest_tf1(x, h, w) if m == 'up'
+         else eo.max_pool_same(x, pool[:2], pool[2:]))
+    res.append(x.permute(0, 2, 3, 1).double())
+  if per_channel:
+    fused = sum(r * torch.from_numpy(np.asarray(cw, np.float64)) for r, cw in zip(res, weights))
+  else:
+    fused = sum(r * float(wt) for r, wt in zip(res, weights))
+  fused = {SWISH: lambda t: t * torch.sigmoid(t), RELU6: lambda t: t.clamp(0, 6),
+           NONE: lambda t: t}[act](fused)
+  return depthwise_f64(fused, taps, 3, 1)
 
 
 def _pool_cases():

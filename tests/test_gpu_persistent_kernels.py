@@ -286,16 +286,25 @@ def test_sepconv(case, impl):
     got = over_grids(launch)
   finally:
     ops.set_option('sepconv_impl', 0)
+  check_sepconv(got, dx, ddw, dpw, db, act, nout, _sep_id(case))
+
+
+def check_sepconv(got, dx, ddw, dpw, db, act, nout, what):
+  """got (host, [N,h,w,ldo]) against edet_fuse_dw + edet_pointwise_conv on the device inputs, bit
+  for bit, and the pair against float64 (see test_sepconv)."""
+  ops = _ops()
+  n, h, w, c = dx.shape
   tmp = Out((n, h, w, c))
-  ops.fuse_dw(spec, ddw, tmp.t, NONE)
-  two = Out((n, h, w, ldo))
+  ops.fuse_dw([(dx, ops.RS_SAME, None, 1.0)], ddw, tmp.t, NONE)
+  two = Out((n, h, w, got.shape[-1]))
   ops.pointwise_conv(tmp.t, dpw, db, two.t, act, rows=n * h * w, nout=nout)
   tmp, two = tmp.result(), two.result()
   assert torch.equal(got[..., :nout], two[..., :nout])
+  x, dw_w, pw, bias = dx.cpu(), ddw.cpu(), dpw.cpu(), db.cpu()
   d = eo.depthwise_conv2d_same(x.double().permute(0, 3, 1, 2), dw_w.double().view(3, 3, c, 1))
   check_close(tmp, d.permute(0, 2, 3, 1), 'depthwise')
   ref = act_ref(tmp.double() @ pw.double().t() + bias.double(), act)
-  check_close(got[..., :nout], ref, _sep_id(case))
+  check_close(got[..., :nout], ref, what)
 
 
 @pytest.mark.parametrize('what', ['c', 'nout', 'ldo'])
