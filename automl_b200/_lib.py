@@ -72,6 +72,8 @@ SIGNATURES = {
     'edet_cls_preprocess': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
                                     c_void_p]),
     'edet_softmax_topk': (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    'edet_seg_masks': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int,
+                               c_int, c_void_p, c_void_p]),
     'edet_pre_nms': (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p),
                              ctypes.POINTER(c_int), c_int, c_int, c_int, c_int, c_int, c_void_p,
                              c_void_p, c_void_p, c_void_p, c_int, c_void_p]),

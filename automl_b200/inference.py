@@ -20,7 +20,9 @@ gives seeded synthetic weights; a path to an .npz whose keys are the reference v
 
 The whole request runs on the device: H2D copy of the uint8 images -> edet_preprocess (images of
 one size) or edet_preprocess_ragged (sizes differ; one launch either way) -> network -> pre-NMS ->
-NMS -> D2H copy of the [N, max_output_size, 7] detections.
+NMS -> D2H copy of the [N, max_output_size, 7] detections.  With 'segmentation' in the config's
+heads, segment_images / segment_stream run the same staging and pre-process, the network without
+NMS, then edet_seg_masks -> one D2H copy of a uint8 mask per image at the image's own size.
 """
 import copy
 import io
@@ -123,6 +125,47 @@ def preprocess_table(shapes, image_size):
   return desc, int(offsets[-1] + nbytes[-1]), np.float32(1.0) / scale
 
 
+def seg_mask_table(shapes, image_size):
+  """The table of ops.seg_masks for images of sizes `shapes` [(h, w), ...] pre-processed to
+  `image_size`: (int32 [N, 6] edet_seg_mask_image rows, packed byte count).  Mask i is the h x w
+  uint8 block at byte offset sum_{j<i} h_j * w_j; scaled_h, scaled_w are the image's size in the
+  letterboxed input, as preprocess_table computes it.  Raises ValueError like preprocess_table."""
+  desc, _, _ = preprocess_table(shapes, image_size)
+  hw = desc[:, 2:4].astype(np.int64)
+  nbytes = hw[:, 0] * hw[:, 1]
+  offsets = np.zeros(len(hw), np.int64)
+  offsets[1:] = np.cumsum(nbytes[:-1])
+  table = np.zeros((len(hw), ops.SEG_MASK_WORDS), np.int32)
+  table[:, :2] = offsets.view(np.int32).reshape(-1, 2)
+  table[:, 2:] = desc[:, 2:]
+  return table, int(offsets[-1] + nbytes[-1])
+
+
+def segment_request(image_arrays, image_size, num_classes):
+  """Checks one segment_images request before anything is enqueued: (shapes [(h, w), ...], mask
+  table, packed byte count).  Raises ValueError for an empty request, an image that is not uint8
+  [h, w, 3] or collapses to zero size, and for more than 256 classes (uint8 masks)."""
+  if not 1 <= num_classes <= ops.SEG_MAX_CLASSES:
+    raise ValueError('seg_num_classes = %d: uint8 masks hold 1..%d classes'
+                     % (num_classes, ops.SEG_MAX_CLASSES))
+  if isinstance(image_arrays, torch.Tensor):
+    if image_arrays.dtype != torch.uint8 or image_arrays.dim() != 4 or image_arrays.shape[3] != 3:
+      raise ValueError('expected a uint8 [N, h, w, 3] tensor, got %s %s'
+                       % (image_arrays.dtype, tuple(image_arrays.shape)))
+    shapes = [tuple(image_arrays.shape[1:3])] * image_arrays.shape[0]
+  else:
+    shapes = []
+    for im in image_arrays:
+      im = np.asarray(im)
+      if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+        raise ValueError('expected uint8 [h, w, 3] images, got %s %s' % (im.dtype, im.shape))
+      shapes.append(im.shape[:2])
+  if not shapes:
+    raise ValueError('empty request')
+  table, total = seg_mask_table(shapes, image_size)
+  return shapes, table, total
+
+
 def _grow(buf, nbytes, **kw):
   """`buf` if it holds `nbytes`, else a new uint8 buffer of at least twice its size."""
   if buf is not None and buf.numel() >= nbytes:
@@ -160,6 +203,33 @@ class _Request(object):
   def result(self):
     """float32 [N (x world), max_output_size, 7] numpy array
     [image_id, ymin, xmin, ymax, xmax, score, class]."""
+    return self._finish()
+
+
+class _SegmentRequest(_Request):
+  """Handle of one in-flight segmentation request (ServingDriver.submit_segment)."""
+
+  def __init__(self, slot, shapes, total):
+    super().__init__(slot)
+    self._shapes, self._total = shapes, total
+
+  def _finish(self):
+    if self._out is None:
+      self._slot['ev_done'].synchronize()
+      packed = self._slot['mask_host'][:self._total].numpy().copy()
+      self._out, off = [], 0
+      for h, w in self._shapes:
+        self._out.append(packed[off:off + h * w].reshape(h, w))
+        off += h * w
+      if self._slot['pending'] is self:
+        self._slot['pending'] = None
+    return self._out
+
+  def done(self):
+    return self._out is not None or self._slot['ev_done'].query()
+
+  def result(self):
+    """List of uint8 [h_i, w_i] numpy masks, one per image: the class of each pixel."""
     return self._finish()
 
 
@@ -208,12 +278,14 @@ class ServingDriver(object):
     self._engines = {}
     self._slots = {}
     self._copy_stream = torch.cuda.Stream(device=self.device)
+    self._d2h_stream = torch.cuda.Stream(device=self.device)   # segmentation masks to the host
     self._seq = 0
     self.engine = self._engine_for(self.batch_size) if self.batch_size else None
     self.signitures = {
         'image_files': 'image_files',     # bytes of encoded images (serve_files)
         'image_arrays': 'image_arrays',   # uint8 HxWx3 arrays (serve_images)
-        'prediction': self.engine.detections if self.engine is not None else 'detections',
+        'prediction': (self.engine.detections if self.engine is not None and
+                       self.engine.arch.has_detection else 'detections'),
     }
     return self.signitures
 
@@ -234,18 +306,25 @@ class ServingDriver(object):
           'gathered': (torch.empty(world * n, eng.max_output_size, 7, device=self.device)
                        if world > 1 else None),
           'raw_host': None, 'raw_dev': None, 'packed_host': None, 'packed_dev': None,
+          'extra_host': None, 'extra_dev': None, 'mask_host': None, 'mask_dev': None,
           'ev_h2d': torch.cuda.Event(), 'ev_raw_free': torch.cuda.Event(),
-          'ev_done': torch.cuda.Event(), 'pending': None,
+          'ev_masks': torch.cuda.Event(), 'ev_done': torch.cuda.Event(), 'pending': None,
       } for _ in range(self.MAX_IN_FLIGHT)]
     return eng
 
   # ---- serving -------------------------------------------------------------------------------
-  def _stage_raw(self, eng, slot, image_arrays):
+  def _stage_raw(self, eng, slot, image_arrays, extra=None):
     """Uploads the uint8 images (copy stream, from pinned memory) and runs the device pre-process
     into the engine input (current stream): images of one size as one [N, h, w, 3] batch, images
     of different sizes packed behind a descriptor table (preprocess_table), checked before anything
-    is enqueued: an image that is not uint8 [h, w, 3] or collapses to zero size raises ValueError."""
+    is enqueued: an image that is not uint8 [h, w, 3] or collapses to zero size raises ValueError.
+
+    extra: None, or an int32 [N, k] table (k even) that travels with the request -- behind the
+    descriptor rows in the same H2D copy for a ragged request, in its own small copy on the copy
+    stream otherwise.  Returns its 8-byte aligned device view (None without it); it stays valid
+    until the slot's next request."""
     n = eng.n
+    extra_dev = None
     main = torch.cuda.current_stream()
     if isinstance(image_arrays, torch.Tensor):   # [N,h,w,3] uint8 (e.g. pinned host memory)
       shapes = {tuple(image_arrays.shape[1:])}
@@ -270,9 +349,17 @@ class ServingDriver(object):
         batch = slot['raw_host']
       if slot['raw_dev'] is None or tuple(slot['raw_dev'].shape) != shape:
         slot['raw_dev'] = torch.empty(shape, dtype=torch.uint8, device=self.device)
+      if extra is not None:
+        slot['ev_h2d'].synchronize()        # the slot's previous H2D has read the staging buffer
+        slot['extra_host'] = _grow(slot['extra_host'], extra.nbytes, pin_memory=True)
+        slot['extra_dev'] = _grow(slot['extra_dev'], extra.nbytes, device=self.device)
+        slot['extra_host'].numpy()[:extra.nbytes] = extra.view(np.uint8).ravel()
+        extra_dev = slot['extra_dev'][:extra.nbytes].view(torch.int32).view(extra.shape)
       with torch.cuda.stream(self._copy_stream):
         self._copy_stream.wait_event(slot['ev_raw_free'])   # pre-process of the request before last
         slot['raw_dev'].copy_(batch, non_blocking=True)
+        if extra is not None:
+          slot['extra_dev'][:extra.nbytes].copy_(slot['extra_host'][:extra.nbytes], non_blocking=True)
         slot['ev_h2d'].record(self._copy_stream)
       main.wait_event(slot['ev_h2d'])
       scale = ops.preprocess(slot['raw_dev'], eng.input, self.mean_rgb, self.stddev_rgb)
@@ -285,7 +372,8 @@ class ServingDriver(object):
           raise ValueError('expected uint8 [h, w, 3] images, got %s %s' % (im.dtype, im.shape))
       desc, total, scales = preprocess_table([im.shape[:2] for im in images],
                                              tuple(eng.input.shape[1:3]))
-      head = (desc.nbytes + 15) // 16 * 16
+      rows = desc.nbytes + (extra.nbytes if extra is not None else 0)   # desc.nbytes: 24 N
+      head = (rows + 15) // 16 * 16
       staged = head + total
       slot['ev_h2d'].synchronize()          # the slot's previous H2D has read the staging buffer
       slot['packed_host'] = _grow(slot['packed_host'], staged, pin_memory=True)
@@ -294,6 +382,9 @@ class ServingDriver(object):
         slot['packed_dev'] = _grow(slot['packed_dev'], staged, device=self.device)
       host, dev = slot['packed_host'].numpy(), slot['packed_dev']
       host[:desc.nbytes] = desc.view(np.uint8).ravel()
+      if extra is not None:
+        host[desc.nbytes:rows] = extra.view(np.uint8).ravel()
+        extra_dev = dev[desc.nbytes:rows].view(torch.int32).view(extra.shape)
       for im, off in zip(images, desc[:, :2].copy().view(np.int64)[:, 0]):
         host[head + off:head + off + im.size] = np.ascontiguousarray(im).reshape(-1)
       with torch.cuda.stream(self._copy_stream):
@@ -306,6 +397,7 @@ class ServingDriver(object):
       slot['ev_raw_free'].record(main)
       slot['scales'].numpy()[:] = scales
     eng.image_scales.copy_(slot['scales'], non_blocking=True)
+    return extra_dev
 
   def submit(self, image_arrays):
     """Enqueues one request and returns a handle; `handle.result()` blocks until its detections
@@ -353,6 +445,78 @@ class ServingDriver(object):
     pending = collections.deque()
     for batch in batches:
       pending.append(self.submit(batch))
+      if len(pending) >= self.MAX_IN_FLIGHT:
+        yield pending.popleft().result()
+    while pending:
+      yield pending.popleft().result()
+
+  # ---- segmentation --------------------------------------------------------------------------
+  def submit_segment(self, image_arrays, resize='nearest'):
+    """Enqueues one segmentation request and returns a handle; `handle.result()` blocks until the
+    masks are in host memory: a list of uint8 [h_i, w_i] numpy arrays, the class of every pixel of
+    each image at its own size.  Needs a config whose `heads` include 'segmentation'.
+
+    The images are staged and pre-processed as in submit() (the mask table rides in the same H2D
+    copy), the network runs without the NMS stage, then one edet_seg_masks launch samples the
+    segmentation logits at the nearest cell of each image's region of the letterboxed input and
+    takes the arg-max over the classes (first class on ties, like tf.argmax in the reference's
+    segmentation demo).  The packed masks reach pinned host memory in one D2H copy on a stream of
+    their own, so up to MAX_IN_FLIGHT requests overlap like detection requests do."""
+    if resize != 'nearest':
+      raise NotImplementedError('mask resize %r: only nearest sampling is built' % (resize,))
+    if torch.distributed.is_available() and torch.distributed.is_initialized():
+      raise NotImplementedError('segmentation masks under torch.distributed are not built')
+    heads = self.params.get('heads') or []
+    if 'segmentation' not in heads:
+      raise ValueError("segmentation masks need 'segmentation' in heads; heads = %s" % (heads,))
+    n = len(image_arrays)
+    if self.batch_size and n != self.batch_size:
+      raise ValueError('expected %d images, got %d' % (self.batch_size, n))
+    if n < 1:
+      raise ValueError('empty request')
+    if getattr(self, '_engines', None) is None:
+      self.build()
+    with torch.cuda.device(self.device):
+      eng = self._engine_for(n)
+      shapes, table, total = segment_request(image_arrays, tuple(eng.input.shape[1:3]),
+                                             int(self.config.seg_num_classes))
+      slot = self._slots[n][self._seq % self.MAX_IN_FLIGHT]
+      self._seq += 1
+      if slot['pending'] is not None:
+        slot['pending']._finish()          # its host buffer is about to be reused
+      dev_table = self._stage_raw(eng, slot, image_arrays, extra=table)
+      main = torch.cuda.current_stream()
+      eng.run(postprocess=False)
+      # the slot's previous request has completed (above), so neither buffer is still in use
+      slot['mask_dev'] = _grow(slot['mask_dev'], total, device=self.device)
+      slot['mask_host'] = _grow(slot['mask_host'], total, pin_memory=True)
+      hs, ws = eng.seg_out.shape[1:3]
+      f = 2 ** (self.config.min_level - 1)
+      assert (hs * f, ws * f) == tuple(eng.input.shape[1:3]), 'logits grid is not input / f'
+      ops.seg_masks(eng.seg_out, self.config.seg_num_classes, f, dev_table,
+                    tuple(int(v) for v in np.max(np.asarray(shapes), axis=0)), slot['mask_dev'])
+      slot['ev_raw_free'].record(main)     # the mask kernel has read the table
+      slot['ev_masks'].record(main)
+      with torch.cuda.stream(self._d2h_stream):
+        self._d2h_stream.wait_event(slot['ev_masks'])
+        slot['mask_host'][:total].copy_(slot['mask_dev'][:total], non_blocking=True)
+        slot['ev_done'].record(self._d2h_stream)
+    handle = _SegmentRequest(slot, [tuple(int(v) for v in s) for s in shapes], total)
+    slot['pending'] = handle
+    return handle
+
+  def segment_images(self, image_arrays, resize='nearest'):
+    """image_arrays: list of HxWx3 uint8 images (sizes may differ) or a uint8 [N, h, w, 3] tensor
+    -> list of uint8 [h_i, w_i] numpy masks, one per image (see submit_segment)."""
+    return self.submit_segment(image_arrays, resize).result()
+
+  def segment_stream(self, batches, resize='nearest'):
+    """Generator over an iterable of requests: yields the masks of each, in order, keeping
+    MAX_IN_FLIGHT requests in flight."""
+    import collections  # pylint: disable=g-import-not-at-top
+    pending = collections.deque()
+    for batch in batches:
+      pending.append(self.submit_segment(batch, resize))
       if len(pending) >= self.MAX_IN_FLIGHT:
         yield pending.popleft().result()
     while pending:

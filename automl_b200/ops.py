@@ -322,6 +322,30 @@ def softmax_topk(logits, probs, classes):
             _ptr(classes, torch.int32), _stream())
 
 
+SEG_MASK_WORDS = 6      # int32 words of one edet_seg_mask_image row: offset (2 words), h, w, scaled_h, scaled_w
+SEG_MAX_CLASSES = 256   # the masks are uint8
+
+
+def seg_masks(logits, num_classes, grid_factor, table, max_hw, out):
+  """Masks at each image's own size in one launch: logits fp16 [N, Hs, Ws, ld] (the segmentation
+  head's output, ld % 8 == 0), table int32 [N, 6] edet_seg_mask_image rows (byte offset of the mask
+  in `out`, h, w, scaled_h, scaled_w; the caller keeps every mask inside `out`), max_hw the largest
+  (h, w) of the table, out uint8 -> out[offset:offset + h*w] = the h x w arg-max mask of each image,
+  sampled at the nearest cell of the letterboxed input (see edet_seg_masks)."""
+  if not 1 <= num_classes <= SEG_MAX_CLASSES:
+    raise ValueError('seg_masks: %d classes do not fit a uint8 mask (1..%d)'
+                     % (num_classes, SEG_MAX_CLASSES))
+  if logits.dim() != 4 or logits.shape[-1] % 8 or logits.shape[-1] < num_classes:
+    raise ValueError('seg_masks: logits %s must be [N, Hs, Ws, ld], ld a multiple of 8 >= %d'
+                     % (tuple(logits.shape), num_classes))
+  n, hs, ws, ld = logits.shape
+  if tuple(table.shape) != (n, SEG_MASK_WORDS):
+    raise ValueError('seg_masks: table %s must be [%d, %d]' % (tuple(table.shape), n, SEG_MASK_WORDS))
+  _lib.call('edet_seg_masks', _ptr(logits, torch.float16), n, hs, ws, ld, num_classes,
+            int(grid_factor), _ptr(table, torch.int32), int(max_hw[0]), int(max_hw[1]),
+            _ptr(out, torch.uint8), _stream())
+
+
 CLASS_ARGMAX_COLS = 96  # columns per anchor of the padded class-head weights (edet_class_argmax)
 
 

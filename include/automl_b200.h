@@ -358,6 +358,31 @@ int edet_softmax_topk(const float* logits, int n, int num_classes, int k, float*
                       int32_t* classes, edet_stream_t stream);
 
 /*
+ * Segmentation masks at each image's own size from the segmentation head's logits, in one launch
+ * for a ragged request.  The reference stops at the logits; its demo takes tf.argmax(pred, -1) at
+ * the network resolution (tf2/segmentation.py:25-27).  Per image i and pixel (y, x) of its h x w
+ * mask, with f = grid_factor (network input size / logits size, 2^(min_level - 1)):
+ *   cell_y = min(((2y + 1) * scaled_h) / (2 * h * f), hs - 1)   (integer division; x alike)
+ *   mask[y, x] = first index of the maximum of logits[i, cell_y, cell_x, 0 .. num_classes)
+ * (np.argmax's rule: fp16 values compared exactly, ties keep the lower class, the first NaN wins).
+ *   logits  half [n, hs, ws, ld] (16-byte aligned), ld % 8 == 0, 1 <= num_classes <= min(ld, 256)
+ *   table   DEVICE edet_seg_mask_image [n] (8-byte aligned): byte offset of the image's mask in
+ *           `out`, its h and w, and its scaled size in the letterboxed input (as in
+ *           edet_preprocess_image); every field positive
+ *   max_h, max_w  the largest h and w of the table (they size the grid)
+ *   out     uint8: mask i is the h x w block at its offset, row-major; nothing else is written
+ * PDL: the table and the logits are read after the wait, so either may come from the launch or
+ * copy before this one.
+ */
+typedef struct {
+  int64_t offset;
+  int32_t h, w, scaled_h, scaled_w;
+} edet_seg_mask_image;
+int edet_seg_masks(const edet_half* logits, int n, int hs, int ws, int ld, int num_classes,
+                   int grid_factor, const edet_seg_mask_image* table, int max_h, int max_w,
+                   uint8_t* out, edet_stream_t stream);
+
+/*
  * Class-predict 1x1 convolution of ONE pyramid level fused with the class half of pre-NMS: the
  * [n, h, w, num_anchors * num_classes] logits are never written; per pixel and anchor the kernel
  * rounds each logit to fp16 (what edet_pointwise_conv would have stored), takes max / first
