@@ -39,6 +39,8 @@ SIGNATURES = {
                                 ctypes.POINTER(c_float), c_void_p]),
     'edet_preprocess_ragged': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                        ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p]),
+    'edet_preprocess_mirrored': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                         ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p]),
     'edet_stem_conv': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                c_int, c_int, c_void_p]),
     'edet_pointwise_conv': (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int,
@@ -87,6 +89,8 @@ SIGNATURES = {
     'edet_per_class_nms': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
                                    c_int, c_int, c_int, c_float, c_float, c_float, c_void_p,
                                    c_void_p, c_void_p, c_void_p, c_void_p]),
+    'edet_wbf': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
+                         c_void_p, c_void_p]),
 }
 
 _lib = None

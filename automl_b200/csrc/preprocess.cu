@@ -3,7 +3,9 @@
 // network input.  Replaces inference.image_preprocess (inference.py:37-56) ->
 // DetectionInputProcessor.normalize_image / set_scale_factors_to_output_size /
 // resize_and_crop_image (dataloader.py:59-65, 115-142).  A ragged request (images of different
-// sizes, batch_image_preprocess inference.py:68-109) is one launch over a descriptor table.
+// sizes, batch_image_preprocess inference.py:68-109) is one launch over a descriptor table.  The
+// mirrored variant also writes each image flipped left to right (test-time augmentation,
+// tf2/postprocess.py:560-573 un-mirrors about the network input width) from the same values.
 // Memory-bound: 3*h*w bytes in, 12*H*W bytes out per image.
 #include "common.cuh"
 
@@ -30,17 +32,22 @@ __device__ __forceinline__ void build_lut(float (&lut)[3][256], float3 mean, flo
 
 // This thread's column of the CTA's kPreRows output rows of one image: `img` is the image's first
 // byte, `o_img` its [out_h, out_w, 3] output.  Both kernels run exactly this, so an image gives the
-// same bits whichever launch it is part of.
+// same bits whichever launch it is part of.  kMirror: each value is also stored at column
+// out_w - 1 - x of `o_mir`, the image's [out_h, out_w, 3] mirrored output.
+template <bool kMirror = false>
 __device__ __forceinline__ void preprocess_rows(const float (&lut)[3][256], const uint8_t* img,
                                                 float* o_img, int h, int w, int out_h, int out_w,
-                                                int scaled_h, int scaled_w) {
+                                                int scaled_h, int scaled_w, float* o_mir = nullptr) {
   const int x = blockIdx.x * 256 + threadIdx.x;
   if (x >= out_w) return;
   const int y_end = min(out_h, static_cast<int>(blockIdx.y + 1) * kPreRows);
   for (int y = blockIdx.y * kPreRows; y < y_end; ++y) {     // the table is shared by kPreRows rows
     float* o = o_img + (static_cast<size_t>(y) * out_w + x) * 3;
+    float* om = nullptr;
+    if constexpr (kMirror) om = o_mir + (static_cast<size_t>(y) * out_w + (out_w - 1 - x)) * 3;
     if (y >= scaled_h || x >= scaled_w) {   // pad_to_bounding_box zero padding
       o[0] = 0.f; o[1] = 0.f; o[2] = 0.f;
+      if constexpr (kMirror) { om[0] = 0.f; om[1] = 0.f; om[2] = 0.f; }
       continue;
     }
     // tf.image.resize bilinear, half_pixel_centers: src = (dst + 0.5) * (in / out) - 0.5
@@ -63,7 +70,9 @@ __device__ __forceinline__ void preprocess_rows(const float (&lut)[3][256], cons
       const float v10 = lut[c][__ldg(p10 + c)], v11 = lut[c][__ldg(p11 + c)];
       const float top = __fadd_rn(v00, __fmul_rn(__fsub_rn(v01, v00), lx));
       const float bot = __fadd_rn(v10, __fmul_rn(__fsub_rn(v11, v10), lx));
-      o[c] = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), ly));
+      const float v = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), ly));
+      o[c] = v;
+      if constexpr (kMirror) om[c] = v;
     }
   }
 }
@@ -97,6 +106,24 @@ preprocess_kernel(const uint8_t* __restrict__ packed, const PreImage* __restrict
   preprocess_rows(lut, packed + d.offset,
                   out + static_cast<size_t>(blockIdx.z) * out_h * out_w * 3, d.h, d.w, out_h, out_w,
                   d.scaled_h, d.scaled_w);
+}
+
+// A ragged request and its mirror: image i of the table to out[i] and, flipped on width, to
+// out[n + i] (`mirror` = n * out_h * out_w * 3 elements further).  Same grid as the ragged launch.
+__global__ void __launch_bounds__(256)
+preprocess_kernel(const uint8_t* __restrict__ packed, const PreImage* __restrict__ desc,
+                  float* __restrict__ out, long long mirror, int out_h, int out_w, float3 mean,
+                  float3 stddev) {
+  __shared__ float lut[3][256];
+  __shared__ PreImage d;
+  if (threadIdx.x < sizeof(PreImage) / 4)
+    reinterpret_cast<int*>(&d)[threadIdx.x] =
+        __ldg(reinterpret_cast<const int*>(desc + blockIdx.z) + threadIdx.x);
+  build_lut(lut, mean, stddev);
+  __syncthreads();
+  float* o_img = out + static_cast<size_t>(blockIdx.z) * out_h * out_w * 3;
+  preprocess_rows<true>(lut, packed + d.offset, o_img, d.h, d.w, out_h, out_w, d.scaled_h,
+                        d.scaled_w, o_img + mirror);
 }
 
 }  // namespace edet
@@ -137,6 +164,26 @@ extern "C" int edet_preprocess_ragged(const uint8_t* packed, const edet_preproce
                  "preprocess_ragged: desc must be 8-byte aligned, out 4-byte aligned");
   preprocess_kernel<<<dim3(ceil_div(out_w, 256), ceil_div(out_h, kPreRows), n), 256, 0, as_stream(stream)>>>(
       packed, reinterpret_cast<const PreImage*>(desc), out, out_h, out_w,
+      make_float3(h_mean_rgb[0], h_mean_rgb[1], h_mean_rgb[2]),
+      make_float3(h_stddev_rgb[0], h_stddev_rgb[1], h_stddev_rgb[2]));
+  EDET_CHECK_LAUNCH();
+  return EDET_OK;
+}
+
+extern "C" int edet_preprocess_mirrored(const uint8_t* packed, const edet_preprocess_image* desc,
+                                        float* out, int n, int out_h, int out_w,
+                                        const float* h_mean_rgb, const float* h_stddev_rgb,
+                                        edet_stream_t stream) {
+  using namespace edet;
+  EDET_CHECK_ARG(packed && desc && out && h_mean_rgb && h_stddev_rgb,
+                 "preprocess_mirrored: null pointer");
+  EDET_CHECK_ARG(n > 0 && n <= 65535 && out_h > 0 && out_w > 0,
+                 "preprocess_mirrored: bad shape (n=%d out=%dx%d)", n, out_h, out_w);
+  EDET_CHECK_ARG(reinterpret_cast<uintptr_t>(desc) % 8 == 0 && reinterpret_cast<uintptr_t>(out) % 4 == 0,
+                 "preprocess_mirrored: desc must be 8-byte aligned, out 4-byte aligned");
+  preprocess_kernel<<<dim3(ceil_div(out_w, 256), ceil_div(out_h, kPreRows), n), 256, 0, as_stream(stream)>>>(
+      packed, reinterpret_cast<const PreImage*>(desc), out,
+      static_cast<long long>(n) * out_h * out_w * 3, out_h, out_w,
       make_float3(h_mean_rgb[0], h_mean_rgb[1], h_mean_rgb[2]),
       make_float3(h_stddev_rgb[0], h_stddev_rgb[1], h_stddev_rgb[2]));
   EDET_CHECK_LAUNCH();

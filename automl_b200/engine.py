@@ -780,6 +780,8 @@ class Engine(LaunchList):
       self.flush()
       main = torch.cuda.current_stream(self.device)
       if self._logits_current:
+        if self._nms_pending[self._cur]:
+          main.wait_event(self._ev_nms[self._cur])   # the NMS that last read this buffer set is done
         (self._pre_ops_full if self._pre_ops_full else self._pre_ops)[self._cur]()
       elif self._head_pending or not self.pipeline:
         main.wait_event(self._ev_pre[self._cur])

@@ -23,6 +23,10 @@ one size) or edet_preprocess_ragged (sizes differ; one launch either way) -> net
 NMS -> D2H copy of the [N, max_output_size, 7] detections.  With 'segmentation' in the config's
 heads, segment_images / segment_stream run the same staging and pre-process, the network without
 NMS, then edet_seg_masks -> one D2H copy of a uint8 mask per image at the image's own size.
+serve_images_tta / serve_stream_tta (flip test-time augmentation) pre-process each image and its
+mirror in one launch (edet_preprocess_mirrored), run the network on the 2N batch, per-class NMS
+(edet_per_class_nms) over all 2N, then weighted box fusion (edet_wbf) -> one D2H copy of the
+clusters.
 """
 import copy
 import io
@@ -233,6 +237,34 @@ class _SegmentRequest(_Request):
     return self._finish()
 
 
+class _TTARequest(_Request):
+  """Handle of one in-flight test-time-augmented request (ServingDriver.submit_tta)."""
+
+  def __init__(self, slot, n, cap):
+    super().__init__(slot)
+    self._n, self._cap = n, cap
+
+  def _finish(self):
+    if self._out is None:
+      self._slot['ev_done'].synchronize()
+      host = self._slot['tta_host'].numpy()
+      size = self._n * self._cap * 7
+      clusters = host[:size].reshape(self._n, self._cap, 7)
+      counts = host[size:size + self._n].view(np.int32)
+      self._out = [clusters[i, :counts[i]].copy() for i in range(self._n)]
+      if self._slot['pending'] is self:
+        self._slot['pending'] = None
+    return self._out
+
+  def done(self):
+    return self._out is not None or self._slot['ev_done'].query()
+
+  def result(self):
+    """List of float32 [k_i, 7] numpy arrays, one per image: [image_id, x1, y1, x2, y2, score,
+    class] rows sorted by score."""
+    return self._finish()
+
+
 class ServingDriver(object):
   """A driver for serving single or batch images (reference inference.py:340)."""
 
@@ -313,7 +345,7 @@ class ServingDriver(object):
     return eng
 
   # ---- serving -------------------------------------------------------------------------------
-  def _stage_raw(self, eng, slot, image_arrays, extra=None):
+  def _stage_raw(self, eng, slot, image_arrays, extra=None, mirrored=False):
     """Uploads the uint8 images (copy stream, from pinned memory) and runs the device pre-process
     into the engine input (current stream): images of one size as one [N, h, w, 3] batch, images
     of different sizes packed behind a descriptor table (preprocess_table), checked before anything
@@ -322,8 +354,14 @@ class ServingDriver(object):
     extra: None, or an int32 [N, k] table (k even) that travels with the request -- behind the
     descriptor rows in the same H2D copy for a ragged request, in its own small copy on the copy
     stream otherwise.  Returns its 8-byte aligned device view (None without it); it stays valid
-    until the slot's next request."""
-    n = eng.n
+    until the slot's next request.
+
+    mirrored: the engine holds 2N images; the N images go through edet_preprocess_mirrored into
+    input[:N] and, flipped on width, input[N:] (a uniform batch through a table of equal rows, in
+    place of `extra`, so a mirrored request takes none), and both halves get the images' scales."""
+    if mirrored and extra is not None:
+      raise ValueError('a mirrored request carries its own descriptor table, not an extra one')
+    n = eng.n // 2 if mirrored else eng.n
     extra_dev = None
     main = torch.cuda.current_stream()
     if isinstance(image_arrays, torch.Tensor):   # [N,h,w,3] uint8 (e.g. pinned host memory)
@@ -349,6 +387,9 @@ class ServingDriver(object):
         batch = slot['raw_host']
       if slot['raw_dev'] is None or tuple(slot['raw_dev'].shape) != shape:
         slot['raw_dev'] = torch.empty(shape, dtype=torch.uint8, device=self.device)
+      if mirrored:                          # image i at byte i * h * w * 3 of raw_dev
+        extra, _, scales = preprocess_table([shape[1:3]] * n, tuple(eng.input.shape[1:3]))
+        extra[:, :2] = (np.arange(n, dtype=np.int64) * int(np.prod(shape[1:]))).view(np.int32).reshape(-1, 2)
       if extra is not None:
         slot['ev_h2d'].synchronize()        # the slot's previous H2D has read the staging buffer
         slot['extra_host'] = _grow(slot['extra_host'], extra.nbytes, pin_memory=True)
@@ -362,11 +403,18 @@ class ServingDriver(object):
           slot['extra_dev'][:extra.nbytes].copy_(slot['extra_host'][:extra.nbytes], non_blocking=True)
         slot['ev_h2d'].record(self._copy_stream)
       main.wait_event(slot['ev_h2d'])
-      scale = ops.preprocess(slot['raw_dev'], eng.input, self.mean_rgb, self.stddev_rgb)
+      if mirrored:
+        ops.preprocess_mirrored(slot['raw_dev'].view(-1), extra_dev, eng.input, self.mean_rgb,
+                                self.stddev_rgb)
+        slot['scales'].numpy()[:] = np.concatenate([scales, scales])
+      else:
+        scale = ops.preprocess(slot['raw_dev'], eng.input, self.mean_rgb, self.stddev_rgb)
+        slot['scales'].fill_(scale)
       slot['ev_raw_free'].record(main)
-      slot['scales'].fill_(scale)
     else:  # ragged batch: descriptor rows, then the packed images; one H2D, one launch
       images = [np.asarray(im) for im in image_arrays]
+      if len(images) != n:
+        raise ValueError('expected %d images, got %d' % (n, len(images)))
       for im in images:
         if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
           raise ValueError('expected uint8 [h, w, 3] images, got %s %s' % (im.dtype, im.shape))
@@ -392,10 +440,11 @@ class ServingDriver(object):
         dev[:staged].copy_(slot['packed_host'][:staged], non_blocking=True)
         slot['ev_h2d'].record(self._copy_stream)
       main.wait_event(slot['ev_h2d'])
-      ops.preprocess_ragged(dev[head:staged], dev[:desc.nbytes].view(torch.int32).view(desc.shape),
-                            eng.input, self.mean_rgb, self.stddev_rgb)
+      (ops.preprocess_mirrored if mirrored else ops.preprocess_ragged)(
+          dev[head:staged], dev[:desc.nbytes].view(torch.int32).view(desc.shape), eng.input,
+          self.mean_rgb, self.stddev_rgb)
       slot['ev_raw_free'].record(main)
-      slot['scales'].numpy()[:] = scales
+      slot['scales'].numpy()[:] = np.concatenate([scales, scales]) if mirrored else scales
     eng.image_scales.copy_(slot['scales'], non_blocking=True)
     return extra_dev
 
@@ -517,6 +566,100 @@ class ServingDriver(object):
     pending = collections.deque()
     for batch in batches:
       pending.append(self.submit_segment(batch, resize))
+      if len(pending) >= self.MAX_IN_FLIGHT:
+        yield pending.popleft().result()
+    while pending:
+      yield pending.popleft().result()
+
+  # ---- flip test-time augmentation --------------------------------------------------------------
+  def submit_tta(self, image_arrays):
+    """Enqueues one horizontal-flip test-time-augmented request and returns a handle;
+    `handle.result()` blocks until the fused detections are in host memory: a list of float32
+    [k_i, 7] numpy arrays [image_id, x1, y1, x2, y2, score, class], sorted by score -- the layout
+    of nms_np / postprocess.generate_detections, not serve_images' [id, y, x, y, x, ...].
+
+    The reference's recipe (tf2/postprocess.py:530-586 with flip=True, tf2/wbf.py:70-95), all on
+    the device: the images are staged as in submit() and edet_preprocess_mirrored writes each
+    letterboxed input and its left-right mirror into the engine of 2N images; the network runs
+    without the NMS stage; pre-NMS and one edet_per_class_nms over all 2N images (nms_configs,
+    image id image_id_base + i and the image's scale for both halves) give nms_np's rows; one
+    edet_wbf launch un-mirrors the second half about image_scale * width and fuses the two models
+    per image.  Only the nms_np branch (nms_configs.pyfunc) is built, as for generate_detections;
+    the TF per-class NMS branch is not.  WBF fuses classes 0 .. num_classes-1 of nms_np's 1-based
+    rows, as the reference does: the last class is dropped and the dummy rows form one class-0
+    cluster at score -1e5.  The clusters reach pinned host memory in one D2H copy on a stream of
+    their own, so up to MAX_IN_FLIGHT requests overlap."""
+    if torch.distributed.is_available() and torch.distributed.is_initialized():
+      raise NotImplementedError('test-time augmentation under torch.distributed is not built')
+    heads = self.params.get('heads')
+    heads = ['object_detection'] if heads is None else list(heads)
+    if 'object_detection' not in heads:
+      raise ValueError("test-time augmentation needs 'object_detection' in heads; heads = %s"
+                       % (heads,))
+    n = len(image_arrays)
+    if self.batch_size and n != self.batch_size:
+      raise ValueError('expected %d images, got %d' % (self.batch_size, n))
+    if n < 1:
+      raise ValueError('empty request')
+    if getattr(self, '_engines', None) is None:
+      self.build()
+    with torch.cuda.device(self.device):
+      eng = self._engine_for(2 * n)
+      slot = self._slots[2 * n][self._seq % self.MAX_IN_FLIGHT]
+      self._seq += 1
+      if slot['pending'] is not None:
+        slot['pending']._finish()          # its buffers are about to be reused
+      self._stage_raw(eng, slot, image_arrays, mirrored=True)
+      nms = self.config.as_dict()['nms_configs']
+      max_out = eng.max_output_size
+      cap = 2 * max_out
+      if slot.get('tta_det') is None:       # the slot's own buffers, reused by its later requests
+        k = eng.total_anchors if not eng.max_nms_inputs else eng.max_nms_inputs
+        ids = np.float32(self.image_id_base) + np.arange(n, dtype=np.float32)
+        size = n * cap * 7 + n
+        slot.update(
+            tta_det=torch.empty(2 * n, max_out, 7, device=self.device),
+            tta_keep=torch.empty(2 * n, max_out, dtype=torch.int32, device=self.device),
+            tta_valid=torch.empty(2 * n, dtype=torch.int32, device=self.device),
+            tta_work=torch.empty(2 * n, k, device=self.device),
+            tta_ids=torch.from_numpy(np.concatenate([ids, ids])).to(self.device),
+            tta_scales=torch.empty(2 * n, device=self.device),
+            tta_out=torch.empty(size, device=self.device),
+            tta_host=torch.empty(size).pin_memory())
+      main = torch.cuda.current_stream()
+      slot['tta_scales'].copy_(slot['scales'], non_blocking=True)
+      eng.run(postprocess=False)
+      ps = eng.pre_nms_only()
+      ops.per_class_nms(ps['boxes'], ps['scores'], ps['classes'], slot['tta_ids'],
+                        slot['tta_scales'], self.config.num_classes, max_out, nms['method'],
+                        nms.get('iou_thresh'), slot['tta_det'], slot['tta_keep'], slot['tta_valid'],
+                        sigma=nms.get('sigma'), score_thresh=nms.get('score_thresh'),
+                        work=slot['tta_work'])
+      out = slot['tta_out']
+      ops.wbf(slot['tta_det'], 2, self.config.num_classes, out[:n * cap * 7].view(n, cap, 7),
+              out[n * cap * 7:].view(torch.int32), mirrored_mask=0b10,
+              image_scales=slot['tta_scales'][:n], width=eng.input.shape[2])
+      slot['ev_masks'].record(main)
+      with torch.cuda.stream(self._d2h_stream):
+        self._d2h_stream.wait_event(slot['ev_masks'])
+        slot['tta_host'].copy_(out, non_blocking=True)
+        slot['ev_done'].record(self._d2h_stream)
+    handle = _TTARequest(slot, n, cap)
+    slot['pending'] = handle
+    return handle
+
+  def serve_images_tta(self, image_arrays):
+    """image_arrays: list of HxWx3 uint8 images (sizes may differ) or a uint8 [N, h, w, 3] tensor
+    -> list of float32 [k_i, 7] numpy arrays of fused detections, one per image (see submit_tta)."""
+    return self.submit_tta(image_arrays).result()
+
+  def serve_stream_tta(self, batches):
+    """Generator over an iterable of requests: yields the fused detections of each, in order,
+    keeping MAX_IN_FLIGHT requests in flight."""
+    import collections  # pylint: disable=g-import-not-at-top
+    pending = collections.deque()
+    for batch in batches:
+      pending.append(self.submit_tta(batch))
       if len(pending) >= self.MAX_IN_FLIGHT:
         yield pending.popleft().result()
     while pending:

@@ -88,6 +88,21 @@ def preprocess_ragged(packed, desc, out, mean_rgb, stddev_rgb):
             _ptr(out, torch.float32), n, oh, ow, mean, std, _stream())
 
 
+def preprocess_mirrored(packed, desc, out, mean_rgb, stddev_rgb):
+  """A request and its mirror in one launch (flip test-time augmentation): packed / desc as
+  preprocess_ragged for N images -> out fp32 [2N,H,W,3], out[:N] as preprocess_ragged writes it and
+  out[N + i] = out[i] flipped on width."""
+  n2, oh, ow = out.shape[0], out.shape[1], out.shape[2]
+  n = n2 // 2
+  if tuple(out.shape) != (2 * n, oh, ow, 3) or n < 1 or tuple(desc.shape) != (n, PRE_DESC_WORDS):
+    raise ValueError('preprocess_mirrored: out %s must be [2N, H, W, 3] and desc %s [N, %d]'
+                     % (tuple(out.shape), tuple(desc.shape), PRE_DESC_WORDS))
+  mean = (ctypes.c_float * 3)(*[float(v) for v in mean_rgb])
+  std = (ctypes.c_float * 3)(*[float(v) for v in stddev_rgb])
+  _lib.call('edet_preprocess_mirrored', _ptr(packed, torch.uint8), _ptr(desc, torch.int32),
+            _ptr(out, torch.float32), n, oh, ow, mean, std, _stream())
+
+
 def stem_conv(images, out, w, bias, act):
   """images fp32 [N,H,W,3] -> out fp16 [N,ceil(H/2),ceil(W/2),C]."""
   n, h, wd, c3 = images.shape
@@ -443,3 +458,28 @@ def per_class_nms(boxes, scores, classes, image_ids, image_scales, num_classes, 
             ctypes.c_float(thr), ctypes.c_float(sig), ctypes.c_float(sth),
             _ptr(work, torch.float32), _ptr(detections, torch.float32),
             _ptr(keep_index, torch.int32), _ptr(num_valid, torch.int32), _stream())
+
+
+WBF_MAX_ROWS = 1024     # EDET_WBF_MAX_ROWS: num_models * rows of one image
+
+
+def wbf(detections, num_models, num_classes, clusters, num_clusters, mirrored_mask=0,
+        image_scales=None, width=1):
+  """Weighted box fusion (tf2/wbf.py ensemble_detections) of every image in one launch:
+  detections fp32 [num_models * N, rows, 7] (model m of image i at block m * N + i, per-class NMS
+  rows [image_id, x1, y1, x2, y2, score, class]) -> clusters fp32 [N, num_models * rows, 7]
+  (sorted by score, then padding rows [0, 0, 0, 0, 0, 0, -1]) and num_clusters i32 [N].  Models
+  whose bit is set in `mirrored_mask` are un-mirrored first about image_scales fp32 [N] * width
+  (see edet_wbf)."""
+  if detections.dim() != 3 or detections.shape[2] != 7 or detections.shape[0] % num_models:
+    raise ValueError('wbf: detections %s must be [num_models * N, rows, 7], num_models = %d'
+                     % (tuple(detections.shape), num_models))
+  n, rows = detections.shape[0] // num_models, detections.shape[1]
+  if tuple(clusters.shape) != (n, num_models * rows, 7) or tuple(num_clusters.shape) != (n,):
+    raise ValueError('wbf: clusters %s must be [%d, %d, 7] and num_clusters %s [%d]'
+                     % (tuple(clusters.shape), n, num_models * rows, tuple(num_clusters.shape), n))
+  if image_scales is not None and tuple(image_scales.shape) != (n,):
+    raise ValueError('wbf: image_scales %s must be [%d]' % (tuple(image_scales.shape), n))
+  _lib.call('edet_wbf', _ptr(detections, torch.float32), n, rows, num_models, int(mirrored_mask),
+            _ptr(image_scales, torch.float32), int(width), int(num_classes),
+            _ptr(clusters, torch.float32), _ptr(num_clusters, torch.int32), _stream())

@@ -137,6 +137,20 @@ int edet_preprocess_ragged(const uint8_t* packed, const edet_preprocess_image* d
                            const float* h_stddev_rgb, edet_stream_t stream);
 
 /*
+ * Serving pre-process of a request and of its horizontal mirror in one launch, for flip test-time
+ * augmentation: the reference un-mirrors the detections of the flipped input about the network
+ * input width (tf2/postprocess.py:560-573, x' = image_scale * width - x), so the mirror is the
+ * letterboxed network input flipped left to right (its zero padding on the left).
+ *   packed, desc, h_mean_rgb, h_stddev_rgb: as edet_preprocess_ragged (a uniform batch is a table
+ *   of equal rows)
+ *   out  float32 [2n, out_h, out_w, 3]: out[i] is what edet_preprocess_ragged writes, bit for bit,
+ *        and out[n + i][y][x] = out[i][y][out_w - 1 - x].  Each pixel is computed once.
+ */
+int edet_preprocess_mirrored(const uint8_t* packed, const edet_preprocess_image* desc, float* out,
+                             int n, int out_h, int out_w, const float* h_mean_rgb,
+                             const float* h_stddev_rgb, edet_stream_t stream);
+
+/*
  * Stem: Conv2D 3x3 stride 2 'same' (3 -> cout, no bias) + BN + act.
  * Replaces backbone/efficientnet_model.py:511-527 (Stem.call).
  *   in   float32 [n, h, w, 3] NHWC            out  half [n, ceil(h/2), ceil(w/2), cout]
@@ -481,6 +495,41 @@ int edet_per_class_nms(const float* boxes, const float* scores, const int32_t* c
                        int num_classes, int max_boxes_to_draw, int method, float iou_thresh,
                        float sigma, float score_thresh, float* work, float* detections,
                        int32_t* keep_index, int32_t* num_valid, edet_stream_t stream);
+
+/*
+ * Weighted box fusion of the per-class NMS rows of several "models" of each image (test-time
+ * augmentation): tf2/wbf.py:19-95 (ensemble_detections with vectorized_iou, find_matching_cluster,
+ * average_detections) applied to concat(model 0 rows, model 1 rows, ...) of each image, in one
+ * launch for the batch.  Replaces the per-image Python loop over TF ops.
+ *   detections float32 [num_models * n, rows, 7] rows [image_id, x1, y1, x2, y2, score, class]:
+ *              model m of image i is block m * n + i (what edet_per_class_nms writes for a batch of
+ *              num_models * n images); num_models * rows <= EDET_WBF_MAX_ROWS
+ *   mirrored_mask  bit m set: model m saw the image mirrored; its rows are first un-mirrored as
+ *              tf2/postprocess.py:560-573 does it, float32 ow = image_scales[i] * width, then
+ *              x1' = ow - x2, x2' = ow - x1
+ *   image_scales float32 [n] (may be NULL when mirrored_mask == 0), width the network input width
+ *   clusters float32 [n, num_models * rows, 7]: the clusters of image i, rows [image_id, x1, y1,
+ *              x2, y2, score, class], then padding rows [0, 0, 0, 0, 0, 0, -1]
+ *   num_clusters int32 [n]
+ * Semantics, float32 throughout with every operation rounded (no FMA contraction):
+ *   - only rows whose class value equals some cid in [0, num_classes) are fused, class by class.
+ *     edet_per_class_nms's classes are 1-based, so class num_classes is dropped and class 0 holds
+ *     its dummy rows [id, 0, 0, 0, 0, -1e5, 0] -- the reference's behaviour, kept for parity;
+ *   - within a class, rows in input order, each matched against the current cluster averages by
+ *     vectorized_iou's order of operations; a new cluster iff max(iou) < 0.55f, else the row joins
+ *     the first index of the maximum (numpy's rule: a NaN IoU, e.g. of zero-area boxes, is the
+ *     maximum and the first NaN wins);
+ *   - a cluster is x = sum(x_j * s_j) / sum(s_j) (sequential sums in join order), score =
+ *     sum(s_j) / count * float32(min(1, count / num_models)), image_id and class of its first row;
+ *   - clusters appended class by class in creation order, then stably sorted by score descending
+ *     (Python's sort(reverse=True)).  NaN scores have no defined place.
+ * An image without a row of a fused class gets 0 clusters (the reference's tf.stack would raise).
+ * PDL: everything is read after the wait, so the rows may come from the launch before this one.
+ */
+#define EDET_WBF_MAX_ROWS 1024
+int edet_wbf(const float* detections, int n, int rows, int num_models, int mirrored_mask,
+             const float* image_scales, int width, int num_classes, float* clusters,
+             int32_t* num_clusters, edet_stream_t stream);
 
 #ifdef __cplusplus
 }
