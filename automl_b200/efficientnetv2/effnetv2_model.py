@@ -34,6 +34,7 @@ import numpy as np
 import torch
 
 from automl_b200 import ops
+from automl_b200 import staging
 from automl_b200 import utils
 from automl_b200.backbone.efficientnet_builder import _layer_namer
 from automl_b200.efficientnetv2 import effnetv2_configs
@@ -403,22 +404,12 @@ class EffNetV2Model(LaunchList):
 
   # ---- classification from decoded images -------------------------------------------------------
   def _cls_slot(self):
-    """The next of two request slots: a pinned staging buffer and its device twin (descriptor rows,
-    then the packed images), the top-k outputs on both sides, and the events ordering their reuse."""
+    """The next of two request slots (_ClassifySlot) and the copy and D2H streams they share."""
     if getattr(self, '_cls', None) is None:
-      n, k = self.n, ops.SOFTMAX_TOPK_MAX_K
       self._cls = {
           'seq': 0, 'copy': torch.cuda.Stream(device=self.device),
           'd2h': torch.cuda.Stream(device=self.device),
-          'slots': [{
-              'host': None, 'dev': None,
-              'probs': torch.empty(n * k, dtype=torch.float32, device=self.device),
-              'classes': torch.empty(n * k, dtype=torch.int32, device=self.device),
-              'host_probs': torch.empty(n * k, dtype=torch.float32).pin_memory(),
-              'host_classes': torch.empty(n * k, dtype=torch.int32).pin_memory(),
-              'ev_h2d': torch.cuda.Event(), 'ev_raw_free': torch.cuda.Event(),
-              'ev_out': torch.cuda.Event(), 'ev_d2h': torch.cuda.Event(),
-          } for _ in range(2)],
+          'slots': [_ClassifySlot(self.n, self.device) for _ in range(2)],
       }
     c = self._cls
     slot = c['slots'][c['seq'] % 2]
@@ -426,61 +417,20 @@ class EffNetV2Model(LaunchList):
     return slot
 
   def _preprocess_into(self, slot, image_arrays):
-    """Stages one request in `slot` (one H2D on the copy stream) and enqueues its pre-process into
-    self.input on the current stream."""
+    """Stages one request in `slot` (staging.StagingSlot.stage: the descriptor rows and the images
+    in one H2D on the copy stream) and enqueues its pre-process into self.input on the current
+    stream."""
     h, w = self.image_size
     if h != w:
       raise ValueError('the classification pre-process needs a square image_size, got %dx%d' % (h, w))
-    n, size = self.n, h
     legacy = preprocessing.is_legacy(self.cfg.data.augname)
-    main = torch.cuda.current_stream(self.device)
-    dev_images = pinned = None
-    if isinstance(image_arrays, torch.Tensor):
-      t = image_arrays
-      if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3:
-        raise ValueError('expected uint8 [N, h, w, 3] images, got %s %s' % (t.dtype, tuple(t.shape)))
-      if t.is_cuda:
-        if t.device != self.input.device:
-          raise ValueError('images are on %s, the model on %s' % (t.device, self.input.device))
-        dev_images = t.contiguous()
-      elif t.is_pinned() and t.is_contiguous():
-        pinned = t
-      images = t if (dev_images is not None or pinned is not None) else list(t.numpy())
-    else:
-      images = [np.asarray(im) for im in image_arrays]
-      for im in images:
-        preprocessing.check_image(im)
-    if len(images) != n:
-      raise ValueError('expected %d images, got %d' % (n, len(images)))
-    shapes = [(int(im.shape[0]), int(im.shape[1])) for im in images]
-    desc, total = preprocessing.image_table(shapes, size, legacy)
-    head = desc.nbytes
-    staged = head + (total if dev_images is None and pinned is None else 0)
-    slot['ev_h2d'].synchronize()              # the slot's previous H2D has read the staging buffer
-    if slot['host'] is None or slot['host'].numel() < staged:
-      slot['host'] = torch.empty(staged, dtype=torch.uint8).pin_memory()
-    need = head + (total if dev_images is None else 0)
-    if slot['dev'] is None or slot['dev'].numel() < need:
-      main.synchronize()                      # nothing in flight still reads the old buffer
-      slot['dev'] = torch.empty(need, dtype=torch.uint8, device=self.device)
-    host = slot['host'].numpy()
-    host[:head] = desc.view(np.uint8).ravel()
-    if staged > head:
-      for im, off in zip(images, desc[:, :2].copy().view(np.int64)[:, 0]):
-        host[head + off:head + off + im.size] = np.ascontiguousarray(im).reshape(-1)
-    dev = slot['dev']
-    with torch.cuda.stream(self._cls['copy']):
-      self._cls['copy'].wait_event(slot['ev_raw_free'])   # the pre-process two requests back is done
-      dev[:staged].copy_(slot['host'][:staged], non_blocking=True)
-      if pinned is not None:
-        dev[head:need].copy_(pinned.view(-1), non_blocking=True)
-      slot['ev_h2d'].record(self._cls['copy'])
-    main.wait_event(slot['ev_h2d'])
-    src = dev_images.view(-1) if dev_images is not None else dev[head:need]
-    ops.cls_preprocess(src, dev[:head].view(torch.int32).view(n, ops.CLS_DESC_WORDS), self.input,
-                       ops.CLS_BICUBIC if legacy else ops.CLS_BILINEAR,
+    request = staging.decoded_images(image_arrays, self.n, self.input.device)
+    desc, _ = preprocessing.image_table(request.shapes, h, legacy)
+    (table,), images = slot.staging.stage(self._cls['copy'], [desc], request,
+                                          desc[:, :2].copy().view(np.int64)[:, 0])
+    ops.cls_preprocess(images, table, self.input, ops.CLS_BICUBIC if legacy else ops.CLS_BILINEAR,
                        preprocessing.device_table(self.device) if legacy else None)
-    slot['ev_raw_free'].record(main)
+    slot.staging.release()
 
   def preprocess(self, image_arrays):
     """Fills self.input from decoded images -- a list of uint8 [h, w, 3] arrays (sizes may differ)
@@ -507,24 +457,17 @@ class EffNetV2Model(LaunchList):
     self.run()
     main = torch.cuda.current_stream(self.device)
     n = self.n
-    probs, classes = slot['probs'][:n * k].view(n, k), slot['classes'][:n * k].view(n, k)
-    main.wait_event(slot['ev_d2h'])           # the slot's previous results have left the device
-    ops.softmax_topk(self.output, probs, classes)
-    slot['ev_out'].record(main)
+    main.wait_event(slot.ev_d2h)              # the slot's previous results have left the device
+    ops.softmax_topk(self.output, slot.probs[:n * k].view(n, k), slot.classes[:n * k].view(n, k))
+    slot.ev_out.record(main)
     d2h = self._cls['d2h']
     with torch.cuda.stream(d2h):
-      d2h.wait_event(slot['ev_out'])
-      slot['host_probs'][:n * k].copy_(slot['probs'][:n * k], non_blocking=True)
-      slot['host_classes'][:n * k].copy_(slot['classes'][:n * k], non_blocking=True)
-      slot['ev_d2h'].record(d2h)
-    slot['k'] = k
+      d2h.wait_event(slot.ev_out)
+      slot.host_probs[:n * k].copy_(slot.probs[:n * k], non_blocking=True)
+      slot.host_classes[:n * k].copy_(slot.classes[:n * k], non_blocking=True)
+      slot.ev_d2h.record(d2h)
+    slot.k = k
     return slot
-
-  def _classify_result(self, slot):
-    slot['ev_d2h'].synchronize()
-    n, k = self.n, slot['k']
-    return (slot['host_probs'][:n * k].numpy().reshape(n, k).copy(),
-            slot['host_classes'][:n * k].numpy().reshape(n, k).copy())
 
   def classify(self, image_arrays, top_k=5):
     """Decoded uint8 images (as `preprocess` takes them) -> (probs float32 [N, top_k], classes
@@ -533,7 +476,7 @@ class EffNetV2Model(LaunchList):
     min(num_classes, 32)."""
     k = self._check_top_k(top_k)
     with torch.cuda.device(self.device):
-      return self._classify_result(self._classify_enqueue(image_arrays, k))
+      return self._classify_enqueue(image_arrays, k).result()
 
   def classify_stream(self, batches, top_k=5):
     """Pipelined `classify` over an iterable of requests, two in flight: the H2D copy of request
@@ -541,14 +484,29 @@ class EffNetV2Model(LaunchList):
     (probs, classes) numpy arrays per request, in order."""
     k = self._check_top_k(top_k)
     with torch.cuda.device(self.device):
-      prev = None
-      for batch in batches:
-        slot = self._classify_enqueue(batch, k)
-        if prev is not None:
-          yield self._classify_result(prev)
-        prev = slot
-      if prev is not None:
-        yield self._classify_result(prev)
+      yield from staging.pipelined(lambda batch: self._classify_enqueue(batch, k), batches, 2)
+
+
+class _ClassifySlot(object):
+  """One of the classifier's two request slots: its staging, the top-k outputs on the device and in
+  pinned memory, and the events ordering their reuse."""
+
+  def __init__(self, n, device):
+    size = n * ops.SOFTMAX_TOPK_MAX_K
+    self.n, self.k = n, None
+    self.staging = staging.StagingSlot(device)
+    self.probs = torch.empty(size, dtype=torch.float32, device=device)
+    self.classes = torch.empty(size, dtype=torch.int32, device=device)
+    self.host_probs = torch.empty(size, dtype=torch.float32).pin_memory()
+    self.host_classes = torch.empty(size, dtype=torch.int32).pin_memory()
+    self.ev_out, self.ev_d2h = torch.cuda.Event(), torch.cuda.Event()
+
+  def result(self):
+    """(probs, classes) numpy [N, k] of the slot's latest request, once they are in host memory."""
+    self.ev_d2h.synchronize()
+    n, k = self.n, self.k
+    return (self.host_probs[:n * k].numpy().reshape(n, k).copy(),
+            self.host_classes[:n * k].numpy().reshape(n, k).copy())
 
 
 def get_model(model_name, model_config=None, include_top=False, weights=None, training=False,

@@ -18,11 +18,13 @@ TensorRT — SURVEY.md section 2 row 8).
 gives seeded synthetic weights; a path to an .npz whose keys are the reference variable names
 (Keras layouts, see weights.py) loads real weights.
 
-The whole request runs on the device: H2D copy of the uint8 images -> edet_preprocess (images of
-one size) or edet_preprocess_ragged (sizes differ; one launch either way) -> network -> pre-NMS ->
-NMS -> D2H copy of the [N, max_output_size, 7] detections.  With 'segmentation' in the config's
-heads, segment_images / segment_stream run the same staging and pre-process, the network without
-NMS, then edet_seg_masks -> one D2H copy of a uint8 mask per image at the image's own size.
+The whole request runs on the device.  Every request kind is checked and staged the same way
+(staging.py): the uint8 images, behind the request's int32 tables, in one H2D copy from a pinned
+buffer of the request's slot, MAX_IN_FLIGHT slots per engine.  Then edet_preprocess (images of one
+size) or edet_preprocess_ragged (sizes differ; one launch either way) -> network -> pre-NMS -> NMS
+-> D2H copy of the [N, max_output_size, 7] detections.  With 'segmentation' in the config's heads,
+segment_images / segment_stream run the same staging and pre-process, the network without NMS,
+then edet_seg_masks -> one D2H copy of a uint8 mask per image at the image's own size.
 serve_images_tta / serve_stream_tta (flip test-time augmentation) pre-process each image and its
 mirror in one launch (edet_preprocess_mirrored), run the network on the 2N batch, per-class NMS
 (edet_per_class_nms) over all 2N, then weighted box fusion (edet_wbf) -> one D2H copy of the
@@ -38,6 +40,7 @@ import torch
 from automl_b200 import hparams_config
 from automl_b200 import ops
 from automl_b200 import parallel
+from automl_b200 import staging
 from automl_b200 import weights as weights_lib
 from automl_b200.arch import DetArch
 from automl_b200.engine import Engine
@@ -145,36 +148,21 @@ def seg_mask_table(shapes, image_size):
   return table, int(offsets[-1] + nbytes[-1])
 
 
-def segment_request(image_arrays, image_size, num_classes):
-  """Checks one segment_images request before anything is enqueued: (shapes [(h, w), ...], mask
-  table, packed byte count).  Raises ValueError for an empty request, an image that is not uint8
-  [h, w, 3] or collapses to zero size, and for more than 256 classes (uint8 masks)."""
+def _mask_classes(num_classes):
+  """`num_classes` if uint8 masks hold that many classes, else ValueError."""
   if not 1 <= num_classes <= ops.SEG_MAX_CLASSES:
     raise ValueError('seg_num_classes = %d: uint8 masks hold 1..%d classes'
                      % (num_classes, ops.SEG_MAX_CLASSES))
-  if isinstance(image_arrays, torch.Tensor):
-    if image_arrays.dtype != torch.uint8 or image_arrays.dim() != 4 or image_arrays.shape[3] != 3:
-      raise ValueError('expected a uint8 [N, h, w, 3] tensor, got %s %s'
-                       % (image_arrays.dtype, tuple(image_arrays.shape)))
-    shapes = [tuple(image_arrays.shape[1:3])] * image_arrays.shape[0]
-  else:
-    shapes = []
-    for im in image_arrays:
-      im = np.asarray(im)
-      if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
-        raise ValueError('expected uint8 [h, w, 3] images, got %s %s' % (im.dtype, im.shape))
-      shapes.append(im.shape[:2])
-  if not shapes:
-    raise ValueError('empty request')
-  table, total = seg_mask_table(shapes, image_size)
-  return shapes, table, total
+  return int(num_classes)
 
 
-def _grow(buf, nbytes, **kw):
-  """`buf` if it holds `nbytes`, else a new uint8 buffer of at least twice its size."""
-  if buf is not None and buf.numel() >= nbytes:
-    return buf
-  return torch.empty(max(nbytes, 2 * buf.numel() if buf is not None else 0), dtype=torch.uint8, **kw)
+def segment_request(image_arrays, image_size, num_classes):
+  """The host checks submit_segment runs on one request before anything is enqueued, without a
+  GPU: (shapes [(h, w), ...], mask table, packed byte count).  Raises ValueError as
+  staging.decoded_images and seg_mask_table do, and for more than 256 classes (uint8 masks)."""
+  _mask_classes(num_classes)
+  shapes = staging.decoded_images(image_arrays).shapes
+  return (shapes,) + seg_mask_table(shapes, image_size)
 
 
 def _rgb3(v):
@@ -184,85 +172,70 @@ def _rgb3(v):
 
 
 class _Request(object):
-  """Handle of one in-flight serving request (ServingDriver.submit)."""
+  """Handle of one in-flight request (ServingDriver.submit, submit_segment, submit_tta): `result()`
+  blocks until the request's results are in its slot's pinned memory and returns `collect(slot)`.
+  `flush` (detection) releases a head / NMS stage the engine may still be holding back."""
 
-  def __init__(self, slot):
-    self._slot = slot
+  def __init__(self, slot, collect, flush=None):
+    self._slot, self._collect, self._flush = slot, collect, flush
     self._out = None
-
-  def _finish(self):
-    if self._out is None:
-      self._slot['engine'].flush()        # a head / NMS stage the engine may still be holding back
-      self._slot['ev_done'].synchronize()
-      self._out = self._slot['host_det'].numpy().copy()
-      if self._slot['pending'] is self:
-        self._slot['pending'] = None
-    return self._out
+    slot.pending = self
 
   def done(self):
-    if self._out is None:
-      self._slot['engine'].flush()
-    return self._out is not None or self._slot['ev_done'].query()
+    if self._out is None and self._flush is not None:
+      self._flush()
+    return self._out is not None or self._slot.ev_done.query()
 
   def result(self):
-    """float32 [N (x world), max_output_size, 7] numpy array
-    [image_id, ymin, xmin, ymax, xmax, score, class]."""
-    return self._finish()
-
-
-class _SegmentRequest(_Request):
-  """Handle of one in-flight segmentation request (ServingDriver.submit_segment)."""
-
-  def __init__(self, slot, shapes, total):
-    super().__init__(slot)
-    self._shapes, self._total = shapes, total
-
-  def _finish(self):
     if self._out is None:
-      self._slot['ev_done'].synchronize()
-      packed = self._slot['mask_host'][:self._total].numpy().copy()
-      self._out, off = [], 0
-      for h, w in self._shapes:
-        self._out.append(packed[off:off + h * w].reshape(h, w))
-        off += h * w
-      if self._slot['pending'] is self:
-        self._slot['pending'] = None
+      if self._flush is not None:
+        self._flush()
+      self._slot.ev_done.synchronize()
+      self._out = self._collect(self._slot)
+      if self._slot.pending is self:
+        self._slot.pending = None
     return self._out
 
-  def done(self):
-    return self._out is not None or self._slot['ev_done'].query()
 
-  def result(self):
-    """List of uint8 [h_i, w_i] numpy masks, one per image: the class of each pixel."""
-    return self._finish()
+class _TTABuffers(object):
+  """The device buffers of a flip TTA request of n images on an engine of 2n: the per-class NMS rows
+  of both views `rows` [2n, max_output_size, 7] with that NMS's `keep`, `valid` and `work` buffers,
+  the image ids and scales of both views, and the fused clusters [n, cap, 7] followed by their int32
+  counts [n] in `fused` (pinned twin `fused_host`)."""
+
+  def __init__(self, eng, image_id_base, device):
+    n, max_out = eng.n // 2, eng.max_output_size
+    self.cap = 2 * max_out
+    k = eng.total_anchors if not eng.max_nms_inputs else eng.max_nms_inputs
+    ids = np.float32(image_id_base) + np.arange(n, dtype=np.float32)
+    size = n * self.cap * 7 + n
+    self.rows = torch.empty(2 * n, max_out, 7, device=device)
+    self.keep = torch.empty(2 * n, max_out, dtype=torch.int32, device=device)
+    self.valid = torch.empty(2 * n, dtype=torch.int32, device=device)
+    self.work = torch.empty(2 * n, k, device=device)
+    self.ids = torch.from_numpy(np.concatenate([ids, ids])).to(device)
+    self.scales = torch.empty(2 * n, device=device)
+    self.fused = torch.empty(size, device=device)
+    self.fused_host = torch.empty(size).pin_memory()
 
 
-class _TTARequest(_Request):
-  """Handle of one in-flight test-time-augmented request (ServingDriver.submit_tta)."""
+class _Slot(object):
+  """One of an engine's MAX_IN_FLIGHT request slots: the request's staging and image scales, its
+  result buffers and the events that order their reuse.  Under batch_size=None, a slot of engine
+  size 2n serves both detection requests of 2n images and TTA requests of n images, so each kind
+  of request keeps result buffers of its own; mask and TTA buffers are allocated on first use."""
 
-  def __init__(self, slot, n, cap):
-    super().__init__(slot)
-    self._n, self._cap = n, cap
-
-  def _finish(self):
-    if self._out is None:
-      self._slot['ev_done'].synchronize()
-      host = self._slot['tta_host'].numpy()
-      size = self._n * self._cap * 7
-      clusters = host[:size].reshape(self._n, self._cap, 7)
-      counts = host[size:size + self._n].view(np.int32)
-      self._out = [clusters[i, :counts[i]].copy() for i in range(self._n)]
-      if self._slot['pending'] is self:
-        self._slot['pending'] = None
-    return self._out
-
-  def done(self):
-    return self._out is not None or self._slot['ev_done'].query()
-
-  def result(self):
-    """List of float32 [k_i, 7] numpy arrays, one per image: [image_id, x1, y1, x2, y2, score,
-    class] rows sorted by score."""
-    return self._finish()
+  def __init__(self, eng, world, device):
+    self.staging = staging.StagingSlot(device)
+    self.scales = torch.empty(eng.n, dtype=torch.float32).pin_memory()
+    self.host_det = torch.empty(world * eng.n, eng.max_output_size, 7).pin_memory()
+    self.gathered = (torch.empty(world * eng.n, eng.max_output_size, 7, device=device)
+                     if world > 1 else None)
+    self.masks_dev = self.masks_host = None    # segmentation: the packed uint8 masks
+    self.tta = None                            # flip TTA: _TTABuffers
+    self.ev_out = torch.cuda.Event()           # after the request's last kernel (masks, TTA)
+    self.ev_done = torch.cuda.Event()          # its results are in pinned memory
+    self.pending = None                        # its handle, until the results are collected
 
 
 class ServingDriver(object):
@@ -310,7 +283,7 @@ class ServingDriver(object):
     self._engines = {}
     self._slots = {}
     self._copy_stream = torch.cuda.Stream(device=self.device)
-    self._d2h_stream = torch.cuda.Stream(device=self.device)   # segmentation masks to the host
+    self._d2h_stream = torch.cuda.Stream(device=self.device)   # mask and TTA results to the host
     self._seq = 0
     self.engine = self._engine_for(self.batch_size) if self.batch_size else None
     self.signitures = {
@@ -329,155 +302,96 @@ class ServingDriver(object):
       world = 1
       if torch.distributed.is_available() and torch.distributed.is_initialized():
         world = torch.distributed.get_world_size()
-      # MAX_IN_FLIGHT requests per batch size: pinned host staging / result buffers, device raw
-      # buffers and the events that order their reuse
-      self._slots[n] = [{
-          'engine': eng,
-          'host_det': torch.empty(world * n, eng.max_output_size, 7).pin_memory(),
-          'scales': torch.empty(n, dtype=torch.float32).pin_memory(),
-          'gathered': (torch.empty(world * n, eng.max_output_size, 7, device=self.device)
-                       if world > 1 else None),
-          'raw_host': None, 'raw_dev': None, 'packed_host': None, 'packed_dev': None,
-          'extra_host': None, 'extra_dev': None, 'mask_host': None, 'mask_dev': None,
-          'ev_h2d': torch.cuda.Event(), 'ev_raw_free': torch.cuda.Event(),
-          'ev_masks': torch.cuda.Event(), 'ev_done': torch.cuda.Event(), 'pending': None,
-      } for _ in range(self.MAX_IN_FLIGHT)]
+      self._slots[n] = [_Slot(eng, world, self.device) for _ in range(self.MAX_IN_FLIGHT)]
     return eng
 
   # ---- serving -------------------------------------------------------------------------------
-  def _stage_raw(self, eng, slot, image_arrays, extra=None, mirrored=False):
-    """Uploads the uint8 images (copy stream, from pinned memory) and runs the device pre-process
-    into the engine input (current stream): images of one size as one [N, h, w, 3] batch, images
-    of different sizes packed behind a descriptor table (preprocess_table), checked before anything
-    is enqueued: an image that is not uint8 [h, w, 3] or collapses to zero size raises ValueError.
+  def _acquire(self, image_arrays, views=1):
+    """Checks one request (staging.decoded_images, against batch_size) and takes the next slot of
+    the engine of `views` x N images, building the driver on first use: (the decoded request, the
+    engine, the slot).  The slot's previous request is completed first, as its buffers are about to
+    be reused.  Nothing is enqueued."""
+    request = staging.decoded_images(image_arrays, self.batch_size or None, self.device)
+    if self._engines is None:
+      self.build()
+    n = views * len(request.shapes)
+    eng = self._engine_for(n)
+    slot = self._slots[n][self._seq % self.MAX_IN_FLIGHT]
+    self._seq += 1
+    if slot.pending is not None:
+      slot.pending.result()
+    return request, eng, slot
 
-    extra: None, or an int32 [N, k] table (k even) that travels with the request -- behind the
-    descriptor rows in the same H2D copy for a ragged request, in its own small copy on the copy
-    stream otherwise.  Returns its 8-byte aligned device view (None without it); it stays valid
-    until the slot's next request.
+  def _stage(self, eng, slot, request, table=None, mirrored=False):
+    """Stages a decoded request in the slot (one H2D on the copy stream) and enqueues its
+    pre-process into the engine input on the current stream:
+      * images of one size: edet_preprocess of the image region viewed [N, h, w, 3];
+      * images of different sizes: edet_preprocess_ragged over the preprocess_table rows;
+      * mirrored (the engine holds 2N images), either kind: edet_preprocess_mirrored into input[:N]
+        and, flipped on width, input[N:]; images of one size take a table of equal rows.
+    Every image's scale goes to the engine, for both halves of a mirrored request.  An image that
+    collapses to zero size raises ValueError from preprocess_table before anything is enqueued; a
+    request of one size that is not mirrored takes no table, and edet_preprocess refuses it.
 
-    mirrored: the engine holds 2N images; the N images go through edet_preprocess_mirrored into
-    input[:N] and, flipped on width, input[N:] (a uniform batch through a table of equal rows, in
-    place of `extra`, so a mirrored request takes none), and both halves get the images' scales."""
-    if mirrored and extra is not None:
-      raise ValueError('a mirrored request carries its own descriptor table, not an extra one')
-    n = eng.n // 2 if mirrored else eng.n
-    extra_dev = None
-    main = torch.cuda.current_stream()
-    if isinstance(image_arrays, torch.Tensor):   # [N,h,w,3] uint8 (e.g. pinned host memory)
-      shapes = {tuple(image_arrays.shape[1:])}
+    table: None, or an int32 [N, k] table that travels with the images for a later kernel.  Returns
+    its device view, and the caller releases the slot's staging after that kernel; without a table
+    the staging is released after the pre-process."""
+    n = len(request.shapes)
+    h, w = request.shapes[0]
+    offsets = np.arange(n, dtype=np.int64) * (h * w * 3)   # one size: an [N, h, w, 3] batch
+    tables = [] if table is None else [table]
+    if mirrored or not request.uniform:
+      desc, _, scales = preprocess_table(request.shapes, tuple(eng.input.shape[1:3]))
+      if request.uniform:
+        desc[:, :2] = offsets.view(np.int32).reshape(-1, 2)
+      offsets = desc[:, :2].copy().view(np.int64)[:, 0]
+      tables.insert(0, desc)
+    views, images = slot.staging.stage(self._copy_stream, tables, request, offsets)
+    if mirrored:
+      ops.preprocess_mirrored(images, views[0], eng.input, self.mean_rgb, self.stddev_rgb)
+      slot.scales.numpy()[:] = np.concatenate([scales, scales])
+    elif request.uniform:
+      slot.scales.fill_(ops.preprocess(images.view(n, h, w, 3), eng.input, self.mean_rgb,
+                                       self.stddev_rgb))
     else:
-      shapes = {tuple(np.shape(im)) for im in image_arrays}
-    if len(shapes) == 1:
-      shape = (n,) + next(iter(shapes))
-      if isinstance(image_arrays, torch.Tensor) and image_arrays.dtype == torch.uint8 and \
-          (image_arrays.is_cuda or image_arrays.is_pinned()):
-        batch = image_arrays
-      else:
-        # stack into this slot's pinned staging buffer (reused; its last H2D must have finished)
-        if slot['raw_host'] is None or tuple(slot['raw_host'].shape) != shape:
-          slot['raw_host'] = torch.empty(shape, dtype=torch.uint8).pin_memory()
-        slot['ev_h2d'].synchronize()
-        host = slot['raw_host'].numpy()
-        if isinstance(image_arrays, torch.Tensor):
-          host[...] = image_arrays.to(torch.uint8).numpy()
-        else:
-          for i, im in enumerate(image_arrays):
-            host[i] = im
-        batch = slot['raw_host']
-      if slot['raw_dev'] is None or tuple(slot['raw_dev'].shape) != shape:
-        slot['raw_dev'] = torch.empty(shape, dtype=torch.uint8, device=self.device)
-      if mirrored:                          # image i at byte i * h * w * 3 of raw_dev
-        extra, _, scales = preprocess_table([shape[1:3]] * n, tuple(eng.input.shape[1:3]))
-        extra[:, :2] = (np.arange(n, dtype=np.int64) * int(np.prod(shape[1:]))).view(np.int32).reshape(-1, 2)
-      if extra is not None:
-        slot['ev_h2d'].synchronize()        # the slot's previous H2D has read the staging buffer
-        slot['extra_host'] = _grow(slot['extra_host'], extra.nbytes, pin_memory=True)
-        slot['extra_dev'] = _grow(slot['extra_dev'], extra.nbytes, device=self.device)
-        slot['extra_host'].numpy()[:extra.nbytes] = extra.view(np.uint8).ravel()
-        extra_dev = slot['extra_dev'][:extra.nbytes].view(torch.int32).view(extra.shape)
-      with torch.cuda.stream(self._copy_stream):
-        self._copy_stream.wait_event(slot['ev_raw_free'])   # pre-process of the request before last
-        slot['raw_dev'].copy_(batch, non_blocking=True)
-        if extra is not None:
-          slot['extra_dev'][:extra.nbytes].copy_(slot['extra_host'][:extra.nbytes], non_blocking=True)
-        slot['ev_h2d'].record(self._copy_stream)
-      main.wait_event(slot['ev_h2d'])
-      if mirrored:
-        ops.preprocess_mirrored(slot['raw_dev'].view(-1), extra_dev, eng.input, self.mean_rgb,
-                                self.stddev_rgb)
-        slot['scales'].numpy()[:] = np.concatenate([scales, scales])
-      else:
-        scale = ops.preprocess(slot['raw_dev'], eng.input, self.mean_rgb, self.stddev_rgb)
-        slot['scales'].fill_(scale)
-      slot['ev_raw_free'].record(main)
-    else:  # ragged batch: descriptor rows, then the packed images; one H2D, one launch
-      images = [np.asarray(im) for im in image_arrays]
-      if len(images) != n:
-        raise ValueError('expected %d images, got %d' % (n, len(images)))
-      for im in images:
-        if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
-          raise ValueError('expected uint8 [h, w, 3] images, got %s %s' % (im.dtype, im.shape))
-      desc, total, scales = preprocess_table([im.shape[:2] for im in images],
-                                             tuple(eng.input.shape[1:3]))
-      rows = desc.nbytes + (extra.nbytes if extra is not None else 0)   # desc.nbytes: 24 N
-      head = (rows + 15) // 16 * 16
-      staged = head + total
-      slot['ev_h2d'].synchronize()          # the slot's previous H2D has read the staging buffer
-      slot['packed_host'] = _grow(slot['packed_host'], staged, pin_memory=True)
-      if slot['packed_dev'] is None or slot['packed_dev'].numel() < staged:
-        main.synchronize()                  # no queued pre-process still reads the old buffer
-        slot['packed_dev'] = _grow(slot['packed_dev'], staged, device=self.device)
-      host, dev = slot['packed_host'].numpy(), slot['packed_dev']
-      host[:desc.nbytes] = desc.view(np.uint8).ravel()
-      if extra is not None:
-        host[desc.nbytes:rows] = extra.view(np.uint8).ravel()
-        extra_dev = dev[desc.nbytes:rows].view(torch.int32).view(extra.shape)
-      for im, off in zip(images, desc[:, :2].copy().view(np.int64)[:, 0]):
-        host[head + off:head + off + im.size] = np.ascontiguousarray(im).reshape(-1)
-      with torch.cuda.stream(self._copy_stream):
-        self._copy_stream.wait_event(slot['ev_raw_free'])   # pre-process of the request before last
-        dev[:staged].copy_(slot['packed_host'][:staged], non_blocking=True)
-        slot['ev_h2d'].record(self._copy_stream)
-      main.wait_event(slot['ev_h2d'])
-      (ops.preprocess_mirrored if mirrored else ops.preprocess_ragged)(
-          dev[head:staged], dev[:desc.nbytes].view(torch.int32).view(desc.shape), eng.input,
-          self.mean_rgb, self.stddev_rgb)
-      slot['ev_raw_free'].record(main)
-      slot['scales'].numpy()[:] = np.concatenate([scales, scales]) if mirrored else scales
-    eng.image_scales.copy_(slot['scales'], non_blocking=True)
-    return extra_dev
+      ops.preprocess_ragged(images, views[0], eng.input, self.mean_rgb, self.stddev_rgb)
+      slot.scales.numpy()[:] = scales
+    if table is None:
+      slot.staging.release()
+    eng.image_scales.copy_(slot.scales, non_blocking=True)
+    return views[-1] if table is not None else None
+
+  def _download(self, slot, dev, host):
+    """After the request's last kernel on the current stream: `dev` to the pinned `host` on the
+    D2H stream, which records the slot's ev_done."""
+    slot.ev_out.record(torch.cuda.current_stream())
+    with torch.cuda.stream(self._d2h_stream):
+      self._d2h_stream.wait_event(slot.ev_out)
+      host.copy_(dev, non_blocking=True)
+      slot.ev_done.record(self._d2h_stream)
 
   def submit(self, image_arrays):
     """Enqueues one request and returns a handle; `handle.result()` blocks until its detections
     are in host memory.  Up to MAX_IN_FLIGHT (3) requests are in flight: the H2D copy and
     pre-process of request i+1, the backbone of request i, the feature network / heads of request
     i-1 and the NMS + D2H copy of request i-1 / i-2 overlap (copy stream, main stream, the engine's
-    head and NMS streams).  Submitting one more request first completes the oldest one."""
-    if getattr(self, '_engines', None) is None:
-      self.build()
-    n = len(image_arrays)
-    if self.batch_size and n != self.batch_size:
-      raise ValueError('expected %d images, got %d' % (self.batch_size, n))
-    if n < 1:
-      raise ValueError('empty request')
+    head and NMS streams).  Submitting one more request first completes the oldest one.
+
+    image_arrays: a list of uint8 [h, w, 3] images (sizes may differ), a uint8 [N, h, w, 3] numpy
+    array or tensor, pinned or not, or such a tensor on the driver's device, which is read in place
+    on the current stream.  Anything else raises ValueError before anything is enqueued."""
     with torch.cuda.device(self.device):
-      eng = self._engine_for(n)
-      slot = self._slots[n][self._seq % self.MAX_IN_FLIGHT]
-      self._seq += 1
-      if slot['pending'] is not None:
-        slot['pending']._finish()          # its host buffer is about to be reused
-      self._stage_raw(eng, slot, image_arrays)
+      request, eng, slot = self._acquire(image_arrays)
+      self._stage(eng, slot, request)
 
       def after_nms(det, slot=slot):
         """On the engine's NMS stream right after NMS: all-gather (multi-GPU) + D2H copy."""
-        det = parallel.gather_detections(det, slot['gathered'])
-        slot['host_det'].copy_(det, non_blocking=True)
-        slot['ev_done'].record(torch.cuda.current_stream())
+        det = parallel.gather_detections(det, slot.gathered)
+        slot.host_det.copy_(det, non_blocking=True)
+        slot.ev_done.record(torch.cuda.current_stream())
       eng.run(postprocess=True, after_nms=after_nms)
-    handle = _Request(slot)
-    slot['pending'] = handle
-    return handle
+    # float32 [N (x world), max_output_size, 7]: [image_id, ymin, xmin, ymax, xmax, score, class]
+    return _Request(slot, lambda s: s.host_det.numpy().copy(), flush=eng.flush)
 
   def serve_images(self, image_arrays):
     """image_arrays: list (or array) of HxWx3 uint8 images -> float32 [N, max_output_size, 7].
@@ -490,20 +404,14 @@ class ServingDriver(object):
   def serve_stream(self, batches):
     """Generator over an iterable of requests: yields the detections of each, in order, keeping
     MAX_IN_FLIGHT requests in flight."""
-    import collections  # pylint: disable=g-import-not-at-top
-    pending = collections.deque()
-    for batch in batches:
-      pending.append(self.submit(batch))
-      if len(pending) >= self.MAX_IN_FLIGHT:
-        yield pending.popleft().result()
-    while pending:
-      yield pending.popleft().result()
+    return staging.pipelined(self.submit, batches, self.MAX_IN_FLIGHT)
 
   # ---- segmentation --------------------------------------------------------------------------
   def submit_segment(self, image_arrays, resize='nearest'):
     """Enqueues one segmentation request and returns a handle; `handle.result()` blocks until the
     masks are in host memory: a list of uint8 [h_i, w_i] numpy arrays, the class of every pixel of
-    each image at its own size.  Needs a config whose `heads` include 'segmentation'.
+    each image at its own size.  Needs a config whose `heads` include 'segmentation' and at most 256
+    classes (uint8 masks).
 
     The images are staged and pre-processed as in submit() (the mask table rides in the same H2D
     copy), the network runs without the NMS stage, then one edet_seg_masks launch samples the
@@ -518,41 +426,29 @@ class ServingDriver(object):
     heads = self.params.get('heads') or []
     if 'segmentation' not in heads:
       raise ValueError("segmentation masks need 'segmentation' in heads; heads = %s" % (heads,))
-    n = len(image_arrays)
-    if self.batch_size and n != self.batch_size:
-      raise ValueError('expected %d images, got %d' % (self.batch_size, n))
-    if n < 1:
-      raise ValueError('empty request')
-    if getattr(self, '_engines', None) is None:
-      self.build()
     with torch.cuda.device(self.device):
-      eng = self._engine_for(n)
-      shapes, table, total = segment_request(image_arrays, tuple(eng.input.shape[1:3]),
-                                             int(self.config.seg_num_classes))
-      slot = self._slots[n][self._seq % self.MAX_IN_FLIGHT]
-      self._seq += 1
-      if slot['pending'] is not None:
-        slot['pending']._finish()          # its host buffer is about to be reused
-      dev_table = self._stage_raw(eng, slot, image_arrays, extra=table)
-      main = torch.cuda.current_stream()
+      request, eng, slot = self._acquire(image_arrays)
+      num_classes = _mask_classes(self.config.seg_num_classes)
+      table, total = seg_mask_table(request.shapes, tuple(eng.input.shape[1:3]))
+      dev_table = self._stage(eng, slot, request, table=table)
       eng.run(postprocess=False)
-      # the slot's previous request has completed (above), so neither buffer is still in use
-      slot['mask_dev'] = _grow(slot['mask_dev'], total, device=self.device)
-      slot['mask_host'] = _grow(slot['mask_host'], total, pin_memory=True)
+      # the slot's previous request has completed (_acquire), so neither buffer is still in use
+      slot.masks_dev = staging.grow(slot.masks_dev, total, device=self.device)
+      slot.masks_host = staging.grow(slot.masks_host, total, pin_memory=True)
       hs, ws = eng.seg_out.shape[1:3]
       f = 2 ** (self.config.min_level - 1)
       assert (hs * f, ws * f) == tuple(eng.input.shape[1:3]), 'logits grid is not input / f'
-      ops.seg_masks(eng.seg_out, self.config.seg_num_classes, f, dev_table,
-                    tuple(int(v) for v in np.max(np.asarray(shapes), axis=0)), slot['mask_dev'])
-      slot['ev_raw_free'].record(main)     # the mask kernel has read the table
-      slot['ev_masks'].record(main)
-      with torch.cuda.stream(self._d2h_stream):
-        self._d2h_stream.wait_event(slot['ev_masks'])
-        slot['mask_host'][:total].copy_(slot['mask_dev'][:total], non_blocking=True)
-        slot['ev_done'].record(self._d2h_stream)
-    handle = _SegmentRequest(slot, [tuple(int(v) for v in s) for s in shapes], total)
-    slot['pending'] = handle
-    return handle
+      ops.seg_masks(eng.seg_out, num_classes, f, dev_table,
+                    tuple(int(v) for v in np.max(request.shapes, axis=0)), slot.masks_dev)
+      slot.staging.release()               # the mask kernel has read the table
+      self._download(slot, slot.masks_dev[:total], slot.masks_host[:total])
+    shapes = request.shapes
+
+    def masks(s):
+      packed = s.masks_host[:total].numpy().copy()
+      offsets = np.cumsum([0] + [h * w for h, w in shapes])
+      return [packed[o:o + h * w].reshape(h, w) for o, (h, w) in zip(offsets, shapes)]
+    return _Request(slot, masks)
 
   def segment_images(self, image_arrays, resize='nearest'):
     """image_arrays: list of HxWx3 uint8 images (sizes may differ) or a uint8 [N, h, w, 3] tensor
@@ -562,14 +458,7 @@ class ServingDriver(object):
   def segment_stream(self, batches, resize='nearest'):
     """Generator over an iterable of requests: yields the masks of each, in order, keeping
     MAX_IN_FLIGHT requests in flight."""
-    import collections  # pylint: disable=g-import-not-at-top
-    pending = collections.deque()
-    for batch in batches:
-      pending.append(self.submit_segment(batch, resize))
-      if len(pending) >= self.MAX_IN_FLIGHT:
-        yield pending.popleft().result()
-    while pending:
-      yield pending.popleft().result()
+    return staging.pipelined(lambda b: self.submit_segment(b, resize), batches, self.MAX_IN_FLIGHT)
 
   # ---- flip test-time augmentation --------------------------------------------------------------
   def submit_tta(self, image_arrays):
@@ -596,57 +485,33 @@ class ServingDriver(object):
     if 'object_detection' not in heads:
       raise ValueError("test-time augmentation needs 'object_detection' in heads; heads = %s"
                        % (heads,))
-    n = len(image_arrays)
-    if self.batch_size and n != self.batch_size:
-      raise ValueError('expected %d images, got %d' % (self.batch_size, n))
-    if n < 1:
-      raise ValueError('empty request')
-    if getattr(self, '_engines', None) is None:
-      self.build()
     with torch.cuda.device(self.device):
-      eng = self._engine_for(2 * n)
-      slot = self._slots[2 * n][self._seq % self.MAX_IN_FLIGHT]
-      self._seq += 1
-      if slot['pending'] is not None:
-        slot['pending']._finish()          # its buffers are about to be reused
-      self._stage_raw(eng, slot, image_arrays, mirrored=True)
+      request, eng, slot = self._acquire(image_arrays, views=2)
+      n = len(request.shapes)
+      self._stage(eng, slot, request, mirrored=True)
+      if slot.tta is None:
+        slot.tta = _TTABuffers(eng, self.image_id_base, self.device)
+      t = slot.tta
       nms = self.config.as_dict()['nms_configs']
-      max_out = eng.max_output_size
-      cap = 2 * max_out
-      if slot.get('tta_det') is None:       # the slot's own buffers, reused by its later requests
-        k = eng.total_anchors if not eng.max_nms_inputs else eng.max_nms_inputs
-        ids = np.float32(self.image_id_base) + np.arange(n, dtype=np.float32)
-        size = n * cap * 7 + n
-        slot.update(
-            tta_det=torch.empty(2 * n, max_out, 7, device=self.device),
-            tta_keep=torch.empty(2 * n, max_out, dtype=torch.int32, device=self.device),
-            tta_valid=torch.empty(2 * n, dtype=torch.int32, device=self.device),
-            tta_work=torch.empty(2 * n, k, device=self.device),
-            tta_ids=torch.from_numpy(np.concatenate([ids, ids])).to(self.device),
-            tta_scales=torch.empty(2 * n, device=self.device),
-            tta_out=torch.empty(size, device=self.device),
-            tta_host=torch.empty(size).pin_memory())
-      main = torch.cuda.current_stream()
-      slot['tta_scales'].copy_(slot['scales'], non_blocking=True)
+      max_out, cap = eng.max_output_size, t.cap
+      t.scales.copy_(slot.scales, non_blocking=True)
       eng.run(postprocess=False)
       ps = eng.pre_nms_only()
-      ops.per_class_nms(ps['boxes'], ps['scores'], ps['classes'], slot['tta_ids'],
-                        slot['tta_scales'], self.config.num_classes, max_out, nms['method'],
-                        nms.get('iou_thresh'), slot['tta_det'], slot['tta_keep'], slot['tta_valid'],
-                        sigma=nms.get('sigma'), score_thresh=nms.get('score_thresh'),
-                        work=slot['tta_work'])
-      out = slot['tta_out']
-      ops.wbf(slot['tta_det'], 2, self.config.num_classes, out[:n * cap * 7].view(n, cap, 7),
-              out[n * cap * 7:].view(torch.int32), mirrored_mask=0b10,
-              image_scales=slot['tta_scales'][:n], width=eng.input.shape[2])
-      slot['ev_masks'].record(main)
-      with torch.cuda.stream(self._d2h_stream):
-        self._d2h_stream.wait_event(slot['ev_masks'])
-        slot['tta_host'].copy_(out, non_blocking=True)
-        slot['ev_done'].record(self._d2h_stream)
-    handle = _TTARequest(slot, n, cap)
-    slot['pending'] = handle
-    return handle
+      ops.per_class_nms(ps['boxes'], ps['scores'], ps['classes'], t.ids, t.scales,
+                        self.config.num_classes, max_out, nms['method'], nms.get('iou_thresh'),
+                        t.rows, t.keep, t.valid, sigma=nms.get('sigma'),
+                        score_thresh=nms.get('score_thresh'), work=t.work)
+      ops.wbf(t.rows, 2, self.config.num_classes, t.fused[:n * cap * 7].view(n, cap, 7),
+              t.fused[n * cap * 7:].view(torch.int32), mirrored_mask=0b10,
+              image_scales=t.scales[:n], width=eng.input.shape[2])
+      self._download(slot, t.fused, t.fused_host)
+
+    def fused(s):
+      host = s.tta.fused_host.numpy()
+      clusters = host[:n * cap * 7].reshape(n, cap, 7)
+      counts = host[n * cap * 7:].view(np.int32)
+      return [clusters[i, :counts[i]].copy() for i in range(n)]
+    return _Request(slot, fused)
 
   def serve_images_tta(self, image_arrays):
     """image_arrays: list of HxWx3 uint8 images (sizes may differ) or a uint8 [N, h, w, 3] tensor
@@ -656,14 +521,7 @@ class ServingDriver(object):
   def serve_stream_tta(self, batches):
     """Generator over an iterable of requests: yields the fused detections of each, in order,
     keeping MAX_IN_FLIGHT requests in flight."""
-    import collections  # pylint: disable=g-import-not-at-top
-    pending = collections.deque()
-    for batch in batches:
-      pending.append(self.submit_tta(batch))
-      if len(pending) >= self.MAX_IN_FLIGHT:
-        yield pending.popleft().result()
-    while pending:
-      yield pending.popleft().result()
+    return staging.pipelined(self.submit_tta, batches, self.MAX_IN_FLIGHT)
 
   def serve_files(self, image_files):
     """image_files: list of encoded image bytes (jpeg/png)."""

@@ -43,11 +43,11 @@ class PerImageDriver(inference.ServingDriver):
   """The ragged path before the staged launch: every image of the request is its own pageable H2D
   copy and its own edet_preprocess launch on the current stream."""
 
-  def _stage_raw(self, eng, slot, image_arrays):
-    for i, im in enumerate(image_arrays):
+  def _stage(self, eng, slot, request, table=None, mirrored=False):
+    for i, im in enumerate(request.images):
       raw = torch.as_tensor(np.ascontiguousarray(im), dtype=torch.uint8).to(self.device)[None]
-      slot['scales'][i] = ops.preprocess(raw, eng.input[i:i + 1], self.mean_rgb, self.stddev_rgb)
-    eng.image_scales.copy_(slot['scales'], non_blocking=True)
+      slot.scales[i] = ops.preprocess(raw, eng.input[i:i + 1], self.mean_rgb, self.stddev_rgb)
+    eng.image_scales.copy_(slot.scales, non_blocking=True)
 
 
 def _gpu():

@@ -26,6 +26,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, HERE)
 from automl_b200 import inference  # noqa: E402
 from automl_b200 import ops  # noqa: E402
+from automl_b200 import staging  # noqa: E402
 from bench_ragged_serving import BATCH, MIX, MODEL, NREQ, SIZE  # noqa: E402
 
 REQS, ROUNDS, WARMUP = 12, 5, 1
@@ -83,17 +84,16 @@ def _time(launch, count):
 def bench_kernels(driver, images):
   n = len(images)
   driver.serve_images_tta(images)
-  slot = next(s for s in driver._slots[2 * n] if s.get('tta_det') is not None)  # pylint: disable=protected-access
+  tta = next(s.tta for s in driver._slots[2 * n] if s.tta is not None)  # pylint: disable=protected-access
   eng = driver._engines[2 * n]                   # pylint: disable=protected-access
   desc, total, _ = inference.preprocess_table([im.shape[:2] for im in images], SIZE)
   packed = np.zeros(total, np.uint8)
-  for im, off in zip(images, desc[:, :2].copy().view(np.int64)[:, 0]):
-    packed[off:off + im.size] = im.reshape(-1)
+  staging.pack(packed, [], images, desc[:, :2].copy().view(np.int64)[:, 0])
   pk, ds = torch.from_numpy(packed).cuda(), torch.from_numpy(desc).cuda()
   mir = torch.empty_like(eng.input)
   nms = driver.config.as_dict()['nms_configs']
   pre = eng.pre_nms_only()
-  det = torch.empty_like(slot['tta_det'])
+  det = torch.empty_like(tta.rows)
   cap = 2 * eng.max_output_size
   clusters = torch.empty(n, cap, 7, device='cuda')
   counts = torch.empty(n, dtype=torch.int32, device='cuda')
@@ -101,19 +101,19 @@ def bench_kernels(driver, images):
       'preprocess_mirrored': lambda: ops.preprocess_mirrored(pk, ds, mir, driver.mean_rgb,
                                                              driver.stddev_rgb),
       'per_class_nms': lambda: ops.per_class_nms(
-          pre['boxes'], pre['scores'], pre['classes'], slot['tta_ids'], slot['tta_scales'],
+          pre['boxes'], pre['scores'], pre['classes'], tta.ids, tta.scales,
           driver.config.num_classes, eng.max_output_size, nms['method'], nms.get('iou_thresh'),
-          det, slot['tta_keep'], slot['tta_valid'], sigma=nms.get('sigma'),
-          score_thresh=nms.get('score_thresh'), work=slot['tta_work']),
+          det, tta.keep, tta.valid, sigma=nms.get('sigma'),
+          score_thresh=nms.get('score_thresh'), work=tta.work),
       'wbf': lambda: ops.wbf(det, 2, driver.config.num_classes, clusters, counts, 0b10,
-                             slot['tta_scales'][:n], SIZE),
+                             tta.scales[:n], SIZE),
   }
   row = {'config': 'D0 %d^2 batch %d -> %d inputs, nms %s, %d anchors, %d rows per model'
                    % (SIZE, n, 2 * n, nms['method'], pre['scores'].shape[1], eng.max_output_size)}
   for name, fn in launches.items():
     row[name + '_us'] = _time(fn, LAUNCHES[name])
   row['preprocess_equals_served_input'] = bool(torch.equal(mir, eng.input))
-  row['nms_equals_served_rows'] = bool(torch.equal(det, slot['tta_det']))
+  row['nms_equals_served_rows'] = bool(torch.equal(det, tta.rows))
   return row
 
 

@@ -156,7 +156,7 @@ def test_driver_stream_of_growing_ragged_requests():
     side = int(60 * 1.3 ** k)
     batches.append([_image(rng, side, side + 17), _image(rng, side + 31, side), _image(rng, side // 2 + 1, side)])
   got = list(driver.serve_stream(batches))
-  assert max(s['packed_dev'].numel() for s in driver._slots[3]) >= sum(im.size for im in batches[-1])
+  assert max(s.staging.dev.numel() for s in driver._slots[3]) >= sum(im.size for im in batches[-1])
   for g, b in zip(got, batches):
     np.testing.assert_array_equal(g, driver.serve_images(b))
 

@@ -136,6 +136,8 @@ def test_pipelined_submit_equals_synchronous_serving():
   # pinned uint8 tensors are uploaded without the host staging copy
   pinned = torch.from_numpy(np.stack(batches[3])).pin_memory()
   np.testing.assert_array_equal(driver.serve_images(pinned), expect[3])
+  # CUDA uint8 tensors are read in place on the current stream
+  np.testing.assert_array_equal(driver.serve_images(pinned.to('cuda:0')), expect[3])
 
 
 def test_dynamic_batch_and_channels_first():

@@ -286,10 +286,10 @@ def test_serve_images_tta_end_to_end():
   images = _rand_images(rng, RAGGED)
   got = drv.serve_images_tta(images)
   n = len(images)
-  slot = [s for s in drv._slots[2 * n] if s.get('tta_det') is not None][-1]  # pylint: disable=protected-access
+  tta = [s.tta for s in drv._slots[2 * n] if s.tta is not None][-1]  # pylint: disable=protected-access
   torch.cuda.synchronize()
-  det = slot['tta_det'].cpu().numpy()
-  scales = slot['tta_scales'].cpu().numpy()
+  det = tta.rows.cpu().numpy()
+  scales = tta.scales.cpu().numpy()
   nc = drv.config.num_classes
   assert len(got) == n
   for i in range(n):
@@ -313,12 +313,14 @@ def test_request_forms_agree():
   together = drv.serve_images_tta(ragged)
   uniform = drv.serve_images_tta(same)
   pinned = drv.serve_images_tta(torch.from_numpy(np.stack(same)).pin_memory())
+  on_device = drv.serve_images_tta(torch.from_numpy(np.stack(same)).to(DEV))
   for i in range(4):
     a = alone[i].copy()
     a[:, 0] = together[i][:, 0]           # image ids follow the position in the request
     assert wo.same_bits(a, together[i]), i
   for i in range(3):
     assert wo.same_bits(uniform[i], together[i]) and wo.same_bits(pinned[i], together[i]), i
+    assert wo.same_bits(on_device[i], uniform[i]), i
 
 
 def test_serve_stream_tta_equals_sequential():

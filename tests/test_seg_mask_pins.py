@@ -107,9 +107,21 @@ def test_op_refuses_class_count_before_any_launch(num_classes):
 ], ids=['float32', 'int16', 'gray', 'rgba', 'float_tensor', 'empty_request', 'empty_image',
         'collapses'])
 def test_invalid_requests_raise(images):
-  from automl_b200 import inference
-  with pytest.raises(ValueError):
-    inference.segment_request(images, 512, 3)
+  """Each entry point's host checks, before anything is enqueued: decoded_images, then the table
+  builder (detection of ragged requests and TTA: preprocess_table, segmentation: segment_request,
+  classification: image_table, with the request's count)."""
+  from automl_b200 import inference, staging
+  from automl_b200.efficientnetv2 import preprocessing
+  forms = {
+      'detection': lambda: inference.preprocess_table(staging.decoded_images(images).shapes, 512),
+      'segmentation': lambda: inference.segment_request(images, 512, 3),
+      'tta': lambda: inference.preprocess_table(staging.decoded_images(images).shapes, 512),
+      'classification': lambda: preprocessing.image_table(
+          staging.decoded_images(images, n=len(images) or 1).shapes, 224, False),
+  }
+  for check in forms.values():
+    with pytest.raises(ValueError):
+      check()
 
 
 def test_detection_only_driver_refuses_masks():
