@@ -356,26 +356,30 @@ class EffNetV2Model(LaunchList):
     of batch i (two copy streams for the two PCIe directions, device staging buffers on both
     sides).  Yields the model output of each batch (what __call__ returns: float32 logits with
     include_top, else the float16 'head_1x1' feature map), in order, as a pinned host tensor
-    that stays valid until two further results have been yielded."""
+    that stays valid until two further results have been yielded.
+
+    The D2H copy of result k is enqueued before result k-1 is yielded, so the pinned results form a
+    ring of three: result k is rewritten by the copy of result k+3, which starts while the caller
+    asks for result k+2."""
     with torch.cuda.device(self.device):
       if getattr(self, '_pipe', None) is None:
         result = self.output
         self._pipe = {
             'in': [torch.empty_like(self.input) for _ in range(2)],
             'out': [torch.empty_like(result) for _ in range(2)],
-            'host': [torch.empty(tuple(result.shape), dtype=result.dtype).pin_memory() for _ in range(2)],
+            'host': [torch.empty(tuple(result.shape), dtype=result.dtype).pin_memory() for _ in range(3)],
             'h2d': torch.cuda.Stream(device=self.device), 'd2h': torch.cuda.Stream(device=self.device),
             'ev_h2d': [torch.cuda.Event() for _ in range(2)],
             'ev_in_free': [torch.cuda.Event() for _ in range(2)],
             'ev_out': [torch.cuda.Event() for _ in range(2)],
-            'ev_d2h': [torch.cuda.Event() for _ in range(2)],
+            'ev_d2h': [torch.cuda.Event() for _ in range(3)],    # one per pinned result
         }
       p = self._pipe
       main = torch.cuda.current_stream(self.device)
       result = self.output
       prev = None
       for k, batch in enumerate(batches):
-        s = k % 2
+        s, h = k % 2, k % 3         # device staging ring of two, pinned results of three
         t = torch.as_tensor(batch)
         if tuple(t.shape) != tuple(self.input.shape):
           raise ValueError('expected input shape %s, got %s' % (tuple(self.input.shape), tuple(t.shape)))
@@ -387,17 +391,17 @@ class EffNetV2Model(LaunchList):
         self.input.copy_(p['in'][s], non_blocking=True)
         p['ev_in_free'][s].record(main)
         self.run()
-        main.wait_event(p['ev_d2h'][s])                  # result k-2 has left this staging buffer
+        main.wait_event(p['ev_d2h'][(k - 2) % 3])        # result k-2 has left this staging buffer
         p['out'][s].copy_(result, non_blocking=True)
         p['ev_out'][s].record(main)
         with torch.cuda.stream(p['d2h']):
           p['d2h'].wait_event(p['ev_out'][s])
-          p['host'][s].copy_(p['out'][s], non_blocking=True)
-          p['ev_d2h'][s].record(p['d2h'])
+          p['host'][h].copy_(p['out'][s], non_blocking=True)
+          p['ev_d2h'][h].record(p['d2h'])
         if prev is not None:
           p['ev_d2h'][prev].synchronize()
           yield p['host'][prev]
-        prev = s
+        prev = h
       if prev is not None:
         p['ev_d2h'][prev].synchronize()
         yield p['host'][prev]
