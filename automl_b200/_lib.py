@@ -41,6 +41,9 @@ SIGNATURES = {
                                        ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p]),
     'edet_preprocess_mirrored': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                          ctypes.POINTER(c_float), ctypes.POINTER(c_float), c_void_p]),
+    'edet_preprocess_float': (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                      ctypes.POINTER(c_float), ctypes.POINTER(c_float),
+                                      ctypes.POINTER(c_float), c_void_p]),
     'edet_stem_conv': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                c_int, c_int, c_void_p]),
     'edet_pointwise_conv': (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int,

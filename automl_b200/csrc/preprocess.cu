@@ -1,12 +1,14 @@
-// Serving pre-process on the device: uint8 HWC image -> (x - mean) / std -> aspect-preserving
-// bilinear resize (TF2 tf.image.resize: half-pixel centres, no antialias) -> zero pad to the
-// network input.  Replaces inference.image_preprocess (inference.py:37-56) ->
-// DetectionInputProcessor.normalize_image / set_scale_factors_to_output_size /
-// resize_and_crop_image (dataloader.py:59-65, 115-142).  A ragged request (images of different
-// sizes, batch_image_preprocess inference.py:68-109) is one launch over a descriptor table.  The
-// mirrored variant also writes each image flipped left to right (test-time augmentation,
-// tf2/postprocess.py:560-573 un-mirrors about the network input width) from the same values.
-// Memory-bound: 3*h*w bytes in, 12*H*W bytes out per image.
+// Serving pre-process on the device: HWC image -> (x - mean) / std -> aspect-preserving bilinear
+// resize (TF2 tf.image.resize: half-pixel centres, no antialias) -> zero pad to the network input.
+// Replaces inference.image_preprocess (inference.py:37-56) and EfficientDetModel._preprocessing
+// (tf2/efficientdet_keras.py:920-954) -> DetectionInputProcessor.normalize_image /
+// set_scale_factors_to_output_size / resize_and_crop_image (dataloader.py:59-65, 115-142), which
+// cast any input to float32 first: uint8 images (serving) and float32 images (the Keras model).  A
+// ragged uint8 request (images of different sizes, batch_image_preprocess inference.py:68-109) is
+// one launch over a descriptor table.  The mirrored variant also writes each image flipped left to
+// right (test-time augmentation, tf2/postprocess.py:560-573 un-mirrors about the network input
+// width) from the same values.
+// Memory-bound: 3*h*w (uint8) or 12*h*w (float32) bytes in, 12*H*W bytes out per image.
 #include "common.cuh"
 
 namespace edet {
@@ -30,14 +32,35 @@ __device__ __forceinline__ void build_lut(float (&lut)[3][256], float3 mean, flo
   }
 }
 
+// Tap loaders: the normalised value of channel c of the pixel at `p`.
+struct LutTaps {                // uint8 images: the CTA's table
+  using T = uint8_t;
+  const float (&lut)[3][256];
+  __device__ __forceinline__ float operator()(const uint8_t* p, int c) const {
+    return lut[c][__ldg(p + c)];
+  }
+};
+
+struct FloatTaps {              // float32 images: the operations that build the table, per tap
+  using T = float;
+  float m[3], sd[3];
+  __device__ __forceinline__ FloatTaps(float3 mean, float3 stddev)
+      : m{mean.x, mean.y, mean.z}, sd{stddev.x, stddev.y, stddev.z} {}
+  __device__ __forceinline__ float operator()(const float* p, int c) const {
+    return __fdiv_rn(__fsub_rn(__ldg(p + c), m[c]), sd[c]);
+  }
+};
+
 // This thread's column of the CTA's kPreRows output rows of one image: `img` is the image's first
-// byte, `o_img` its [out_h, out_w, 3] output.  Both kernels run exactly this, so an image gives the
-// same bits whichever launch it is part of.  kMirror: each value is also stored at column
-// out_w - 1 - x of `o_mir`, the image's [out_h, out_w, 3] mirrored output.
-template <bool kMirror = false>
-__device__ __forceinline__ void preprocess_rows(const float (&lut)[3][256], const uint8_t* img,
+// element, `o_img` its [out_h, out_w, 3] output.  Every kernel runs exactly this, so an image gives
+// the same bits whichever launch it is part of, and a float32 image of integral values 0..255 the
+// bits of the same uint8 image.  kMirror: each value is also stored at column out_w - 1 - x of
+// `o_mir`, the image's [out_h, out_w, 3] mirrored output.
+template <bool kMirror = false, class Taps>
+__device__ __forceinline__ void preprocess_rows(const Taps& taps, const typename Taps::T* img,
                                                 float* o_img, int h, int w, int out_h, int out_w,
                                                 int scaled_h, int scaled_w, float* o_mir = nullptr) {
+  using T = typename Taps::T;
   const int x = blockIdx.x * 256 + threadIdx.x;
   if (x >= out_w) return;
   const int y_end = min(out_h, static_cast<int>(blockIdx.y + 1) * kPreRows);
@@ -59,15 +82,15 @@ __device__ __forceinline__ void preprocess_rows(const float (&lut)[3][256], cons
     const int y0 = max(static_cast<int>(fy0), 0), y1 = min(static_cast<int>(ceilf(fy)), h - 1);
     const int x0 = max(static_cast<int>(fx0), 0), x1 = min(static_cast<int>(ceilf(fx)), w - 1);
     const float ly = __fsub_rn(fy, fy0), lx = __fsub_rn(fx, fx0);
-    const uint8_t* p00 = img + (static_cast<size_t>(y0) * w + x0) * 3;
-    const uint8_t* p01 = img + (static_cast<size_t>(y0) * w + x1) * 3;
-    const uint8_t* p10 = img + (static_cast<size_t>(y1) * w + x0) * 3;
-    const uint8_t* p11 = img + (static_cast<size_t>(y1) * w + x1) * 3;
+    const T* p00 = img + (static_cast<size_t>(y0) * w + x0) * 3;
+    const T* p01 = img + (static_cast<size_t>(y0) * w + x1) * 3;
+    const T* p10 = img + (static_cast<size_t>(y1) * w + x0) * 3;
+    const T* p11 = img + (static_cast<size_t>(y1) * w + x1) * 3;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       // normalise first (as the reference does), then interpolate
-      const float v00 = lut[c][__ldg(p00 + c)], v01 = lut[c][__ldg(p01 + c)];
-      const float v10 = lut[c][__ldg(p10 + c)], v11 = lut[c][__ldg(p11 + c)];
+      const float v00 = taps(p00, c), v01 = taps(p01, c);
+      const float v10 = taps(p10, c), v11 = taps(p11, c);
       const float top = __fadd_rn(v00, __fmul_rn(__fsub_rn(v01, v00), lx));
       const float bot = __fadd_rn(v10, __fmul_rn(__fsub_rn(v11, v10), lx));
       const float v = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), ly));
@@ -86,7 +109,7 @@ preprocess_kernel(const uint8_t* __restrict__ in, float* __restrict__ out, int h
   build_lut(lut, mean, stddev);
   __syncthreads();
   const int img = blockIdx.z;
-  preprocess_rows(lut, in + static_cast<size_t>(img) * h * w * 3,
+  preprocess_rows(LutTaps{lut}, in + static_cast<size_t>(img) * h * w * 3,
                   out + static_cast<size_t>(img) * out_h * out_w * 3, h, w, out_h, out_w, scaled_h,
                   scaled_w);
 }
@@ -103,7 +126,7 @@ preprocess_kernel(const uint8_t* __restrict__ packed, const PreImage* __restrict
         __ldg(reinterpret_cast<const int*>(desc + blockIdx.z) + threadIdx.x);
   build_lut(lut, mean, stddev);
   __syncthreads();
-  preprocess_rows(lut, packed + d.offset,
+  preprocess_rows(LutTaps{lut}, packed + d.offset,
                   out + static_cast<size_t>(blockIdx.z) * out_h * out_w * 3, d.h, d.w, out_h, out_w,
                   d.scaled_h, d.scaled_w);
 }
@@ -122,8 +145,30 @@ preprocess_kernel(const uint8_t* __restrict__ packed, const PreImage* __restrict
   build_lut(lut, mean, stddev);
   __syncthreads();
   float* o_img = out + static_cast<size_t>(blockIdx.z) * out_h * out_w * 3;
-  preprocess_rows<true>(lut, packed + d.offset, o_img, d.h, d.w, out_h, out_w, d.scaled_h,
-                        d.scaled_w, o_img + mirror);
+  preprocess_rows<true>(LutTaps{lut}, packed + d.offset, o_img, d.h, d.w, out_h, out_w,
+                        d.scaled_h, d.scaled_w, o_img + mirror);
+}
+
+// A float32 batch of one size: the same grid as the uint8 launch, no table -- each tap is
+// normalised where it is read (FloatTaps).  NaN and Inf pass through the arithmetic.
+__global__ void __launch_bounds__(256)
+preprocess_kernel(const float* __restrict__ in, float* __restrict__ out, int h, int w,
+                  int out_h, int out_w, int scaled_h, int scaled_w, float3 mean, float3 stddev) {
+  const int img = blockIdx.z;
+  preprocess_rows(FloatTaps(mean, stddev), in + static_cast<size_t>(img) * h * w * 3,
+                  out + static_cast<size_t>(img) * out_h * out_w * 3, h, w, out_h, out_w, scaled_h,
+                  scaled_w);
+}
+
+// dataloader.py:115-127 (float32 arithmetic, truncation to int): the scale that fits an h x w
+// image into out_h x out_w, and the scaled size.
+static float fit_scale(int h, int w, int out_h, int out_w, int* scaled_h, int* scaled_w) {
+  const float sy = static_cast<float>(out_h) / static_cast<float>(h);
+  const float sx = static_cast<float>(out_w) / static_cast<float>(w);
+  const float image_scale = sx < sy ? sx : sy;
+  *scaled_h = static_cast<int>(static_cast<float>(h) * image_scale);
+  *scaled_w = static_cast<int>(static_cast<float>(w) * image_scale);
+  return image_scale;
 }
 
 }  // namespace edet
@@ -134,12 +179,8 @@ extern "C" int edet_preprocess(const uint8_t* in, float* out, int n, int h, int 
   using namespace edet;
   EDET_CHECK_ARG(in && out && h_mean_rgb && h_stddev_rgb, "preprocess: null pointer");
   EDET_CHECK_ARG(n > 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "preprocess: bad shape");
-  // dataloader.py:115-127 (float32 arithmetic, truncation to int)
-  const float sy = static_cast<float>(out_h) / static_cast<float>(h);
-  const float sx = static_cast<float>(out_w) / static_cast<float>(w);
-  const float image_scale = sx < sy ? sx : sy;
-  const int scaled_h = static_cast<int>(static_cast<float>(h) * image_scale);
-  const int scaled_w = static_cast<int>(static_cast<float>(w) * image_scale);
+  int scaled_h, scaled_w;
+  const float image_scale = fit_scale(h, w, out_h, out_w, &scaled_h, &scaled_w);
   EDET_CHECK_ARG(scaled_h > 0 && scaled_w > 0, "preprocess: image collapses to zero size");
   if (h_image_scale) *h_image_scale = 1.0f / image_scale;   // image_scale_to_original
   EDET_CHECK_ARG(n <= 65535, "preprocess: n must be <= 65535");
@@ -184,6 +225,27 @@ extern "C" int edet_preprocess_mirrored(const uint8_t* packed, const edet_prepro
   preprocess_kernel<<<dim3(ceil_div(out_w, 256), ceil_div(out_h, kPreRows), n), 256, 0, as_stream(stream)>>>(
       packed, reinterpret_cast<const PreImage*>(desc), out,
       static_cast<long long>(n) * out_h * out_w * 3, out_h, out_w,
+      make_float3(h_mean_rgb[0], h_mean_rgb[1], h_mean_rgb[2]),
+      make_float3(h_stddev_rgb[0], h_stddev_rgb[1], h_stddev_rgb[2]));
+  EDET_CHECK_LAUNCH();
+  return EDET_OK;
+}
+
+extern "C" int edet_preprocess_float(const float* in, float* out, int n, int h, int w, int out_h,
+                                     int out_w, const float* h_mean_rgb, const float* h_stddev_rgb,
+                                     float* h_image_scale, edet_stream_t stream) {
+  using namespace edet;
+  EDET_CHECK_ARG(in && out && h_mean_rgb && h_stddev_rgb, "preprocess_float: null pointer");
+  EDET_CHECK_ARG(n > 0 && n <= 65535 && h > 0 && w > 0 && out_h > 0 && out_w > 0,
+                 "preprocess_float: bad shape (n=%d in=%dx%d out=%dx%d)", n, h, w, out_h, out_w);
+  EDET_CHECK_ARG(reinterpret_cast<uintptr_t>(in) % 4 == 0 && reinterpret_cast<uintptr_t>(out) % 4 == 0,
+                 "preprocess_float: in and out must be 4-byte aligned");
+  int scaled_h, scaled_w;
+  const float image_scale = fit_scale(h, w, out_h, out_w, &scaled_h, &scaled_w);
+  EDET_CHECK_ARG(scaled_h > 0 && scaled_w > 0, "preprocess_float: image collapses to zero size");
+  if (h_image_scale) *h_image_scale = 1.0f / image_scale;   // image_scale_to_original
+  preprocess_kernel<<<dim3(ceil_div(out_w, 256), ceil_div(out_h, kPreRows), n), 256, 0, as_stream(stream)>>>(
+      in, out, h, w, out_h, out_w, scaled_h, scaled_w,
       make_float3(h_mean_rgb[0], h_mean_rgb[1], h_mean_rgb[2]),
       make_float3(h_stddev_rgb[0], h_stddev_rgb[1], h_stddev_rgb[2]));
   EDET_CHECK_LAUNCH();

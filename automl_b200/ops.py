@@ -70,6 +70,25 @@ def preprocess(raw, out, mean_rgb, stddev_rgb):
   return scale.value
 
 
+def preprocess_float(images, out, mean_rgb, stddev_rgb):
+  """images float32 [N,h,w,3] -> out float32 [N,H,W,3], as `preprocess` computes it for uint8
+  images (an image of integral values 0..255 gives the same bits); returns
+  image_scale_to_original (float).  Refuses other dtypes, shapes and strides before launching."""
+  if images.dim() != 4 or images.shape[-1] != 3 or out.dim() != 4 or out.shape[-1] != 3:
+    raise ValueError('preprocess_float: images %s and out %s must be [N, h, w, 3] and [N, H, W, 3]'
+                     % (tuple(images.shape), tuple(out.shape)))
+  n, h, w, _ = images.shape
+  _, oh, ow, _ = out.shape
+  if out.shape[0] != n:
+    raise ValueError('preprocess_float: %d images, out holds %d' % (n, out.shape[0]))
+  mean = (ctypes.c_float * 3)(*[float(v) for v in mean_rgb])
+  std = (ctypes.c_float * 3)(*[float(v) for v in stddev_rgb])
+  scale = ctypes.c_float(0.0)
+  _lib.call('edet_preprocess_float', _ptr(images, torch.float32), _ptr(out, torch.float32), n, h, w,
+            oh, ow, mean, std, ctypes.byref(scale), _stream())
+  return scale.value
+
+
 PRE_DESC_WORDS = 6      # int32 words of one edet_preprocess_image row: offset (2 words), h, w, scaled_h, scaled_w
 
 

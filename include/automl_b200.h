@@ -151,6 +151,19 @@ int edet_preprocess_mirrored(const uint8_t* packed, const edet_preprocess_image*
                              const float* h_stddev_rgb, edet_stream_t stream);
 
 /*
+ * Serving pre-process of float32 images (all the same size): edet_preprocess with each tap
+ * normalised as it is read, (x - mean) / std in float32, the operations edet_preprocess's table is
+ * built with -- an image of integral values 0..255 gives edet_preprocess's bits for the same uint8
+ * image.  Replaces EfficientDetModel._preprocessing tf2/efficientdet_keras.py:920-954 for float
+ * input (dataloader.py:59-65 casts any image to float32).  NaN and Inf pass through.
+ *   in  float32 [n, h, w, 3]   out float32 [n, out_h, out_w, 3]   (both 4-byte aligned)
+ *   h_mean_rgb / h_stddev_rgb: HOST float32[3];  h_image_scale: HOST out, as edet_preprocess
+ */
+int edet_preprocess_float(const float* in, float* out, int n, int h, int w, int out_h, int out_w,
+                          const float* h_mean_rgb, const float* h_stddev_rgb, float* h_image_scale,
+                          edet_stream_t stream);
+
+/*
  * Stem: Conv2D 3x3 stride 2 'same' (3 -> cout, no bias) + BN + act.
  * Replaces backbone/efficientnet_model.py:511-527 (Stem.call).
  *   in   float32 [n, h, w, 3] NHWC            out  half [n, ceil(h/2), ceil(w/2), cout]
