@@ -5,13 +5,15 @@
   * allocates every activation buffer once (NHWC fp16, static shapes);
   * records the launch list (stem -> MBConv blocks -> extra levels -> BiFPN cells -> heads ->
     pre-NMS -> NMS) and replays it as CUDA graphs: the whole network as one graph for forward(),
-    three overlapping stages on three streams for run(postprocess=True) (backbone of step i+1 over
-    feature network + heads + pre-NMS of step i over NMS of step i; Engine._run_pipelined).
+    one pipelined step of three overlapping stages on three streams for run(postprocess=True)
+    (backbone of step i+1 over feature network + heads + pre-NMS of step i over NMS of step i;
+    Engine._run_pipelined).
 
 The launch list mirrors the call structure of efficientdet_arch.efficientdet
 (/root/reference/efficientdet/efficientdet_arch.py:547-577) and inference.det_post_process
 (inference.py:233-271).  PyTorch is used for device memory, streams and graph capture only.
 """
+import contextlib
 import math
 import os
 
@@ -51,8 +53,7 @@ class Engine(LaunchList):
 
   def __init__(self, config, weights, batch_size, device='cuda:0', pw_impl=ops.PW_TCGEN05,
                use_cuda_graph=True, image_id_base=0, fuse_mbconv_front=False,
-               fuse_sepconv=True, pipeline=True, defer_heads=False,
-               fuse_class_argmax=True):
+               fuse_sepconv=True, pipeline=True, fuse_class_argmax=True):
     if not torch.cuda.is_available():
       raise RuntimeError('automl_b200.Engine needs a CUDA device; there is no CPU fallback')
     self.config = config
@@ -71,10 +72,6 @@ class Engine(LaunchList):
     if os.environ.get('EDET_PIPELINE'):        # A/B switch for scripts / bench runs
       pipeline = os.environ['EDET_PIPELINE'] != '0'
     self.pipeline = pipeline
-    if os.environ.get('EDET_DEFER_HEADS'):
-      defer_heads = os.environ['EDET_DEFER_HEADS'] != '0'
-    self.defer_heads = bool(defer_heads and pipeline)   # see _run_pipelined
-    self._deferred = None
     # run(postprocess=True): the class-predict 1x1 conv computes max / arg-max / sigmoid over the
     # classes in its epilogue (edet_class_argmax) and never writes the [N,H,W,810] logits;
     # forward() always writes them.  Bit-identical detections either way.
@@ -130,16 +127,6 @@ class Engine(LaunchList):
     first = next((b for b in a.blocks if b.reduction and b.reduction >= a.config.min_level), None)
     self._bb_split = (self.op_names().index(first.name + '/project') if first else
                       self.num_backbone_ops)
-    if self.defer_heads:
-      # the held-back head stage reads copies of P3..P5 (see _run_pipelined); torch's copy kernel
-      for level in sorted(feats):
-        if level >= a.config.min_level:
-          src = feats[level]
-          dst = self._buf('P%d_copy' % level, tuple(src.shape))
-          self._add('feat_copy/P%d' % level, lambda src=src, dst=dst: dst.copy_(src),
-                    kind='memcpy', nbytes=4 * src.numel(), kernels=0)
-          feats[level] = dst
-    self._heads_start = len(self._ops)
 
     # -- feature network --------------------------------------------------------------------
     F = a.fpn_filters
@@ -439,16 +426,13 @@ class Engine(LaunchList):
     self._scales_ring = [self._buf('image_scales_ring%d' % i, (n,), f32) for i in range(4)]
     for t in self._scales_ring:
       t.fill_(1.0)
-    # Stream priorities of the head and NMS stages (A/B switches).  Measured on the D0 step: a
+    # The head and NMS streams keep the default priority.  Measured on a B200 D0 step: a
     # high-priority head stage pushes whole waves of the next backbone out (4.04 ms), equal
-    # priorities let it fill the slots the backbone leaves (3.90 ms).
-    self._head_priority = -1 if os.environ.get('EDET_HEAD_PRIO', '0') != '0' else 0
-    self._nms_priority = -1 if os.environ.get('EDET_NMS_PRIO', '0') != '0' else 0
-    self._nms_stream = torch.cuda.Stream(device=self.device, priority=self._nms_priority)
-    self._head_stream = torch.cuda.Stream(device=self.device, priority=self._head_priority)
-    self._head_capture_stream = torch.cuda.Stream(device=self.device, priority=self._head_priority)
+    # priorities let it fill the slots the backbone leaves (3.89 ms).
+    self._nms_stream = torch.cuda.Stream(device=self.device)
+    self._head_stream = torch.cuda.Stream(device=self.device)
+    self._head_capture_stream = torch.cuda.Stream(device=self.device)
     self._ev_bb = torch.cuda.Event()
-    self._ev_early = torch.cuda.Event()
     self._ev_head = torch.cuda.Event()
     self._head_pending = False
     self._ev_pre = [torch.cuda.Event() for _ in range(2)]
@@ -502,11 +486,10 @@ class Engine(LaunchList):
     self._branch = None
 
   # ---- execution ------------------------------------------------------------------------------
-  def _run_ops(self, upto=None, parallel_branches=True, start=0, priority=0):
+  def _run_ops(self, upto=None, parallel_branches=True, start=0):
     """Runs ops [start, upto) of the launch list on the current stream; ops tagged with a branch
     run on side streams forked from / joined back into it (parallel graph branches when
-    captured).  priority: CUDA priority of the side streams (the head half of a pipelined step
-    runs at high priority so that its short kernels are not queued behind the next backbone)."""
+    captured)."""
     upto = len(self._ops) if upto is None else upto
     main = torch.cuda.current_stream(self.device)
     open_branches = {}
@@ -523,10 +506,9 @@ class Engine(LaunchList):
         continue
       st = open_branches.get(br)
       if st is None:
-        st = self._branch_streams.get((br, priority))
+        st = self._branch_streams.get(br)
         if st is None:
-          st = self._branch_streams[(br, priority)] = torch.cuda.Stream(device=self.device,
-                                                                        priority=priority)
+          st = self._branch_streams[br] = torch.cuda.Stream(device=self.device)
         st.wait_stream(main)                   # fork
         open_branches[br] = st
       with torch.cuda.stream(st):
@@ -580,26 +562,24 @@ class Engine(LaunchList):
     """Enqueues one forward from self.input.
 
     postprocess=False: network only, on the current stream (writes every head output).
-    postprocess=True : backbone on the current stream, feature network + heads + pre-NMS on the
-      engine's head stream, NMS (and `after_nms(dets)`, e.g. the all-gather / D2H copy) on its NMS
-      stream, so consecutive steps overlap (pipeline=False: network + pre-NMS as one graph on the
-      current stream, only the NMS overlaps the next step).  The class logits are not stored on
-      this path (fuse_class_argmax).  Call wait_detections() (or detect()) before reading
-      `self.detections` from the current stream.
+    postprocess=True : one pipelined step (_run_pipelined): backbone on the current stream,
+      feature network + heads + pre-NMS on the engine's head stream, NMS (and `after_nms(dets)`,
+      e.g. the all-gather / D2H copy) on its NMS stream, so consecutive steps overlap
+      (pipeline=False: network + pre-NMS as one graph on the current stream, only the NMS overlaps
+      the next step).  The class logits are not stored on this path (fuse_class_argmax).  Call
+      wait_detections() (or detect()) before reading `self.detections` from the current stream.
     """
-    net_upto = self.num_network_ops
     if postprocess and not self.arch.has_detection:
       raise ValueError('post-processing needs the object_detection head; config.heads = %s'
                        % (self.arch.heads,))
     if not postprocess:
-      self.flush()
       self._logits_current = True
       if self._head_pending:   # a pipelined step may still be reading / writing the head buffers
         torch.cuda.current_stream(self.device).wait_event(self._ev_pre[self._cur])
       if self.use_cuda_graph:
-        self._graph_for('net', lambda: self._run_ops(net_upto)).replay()
+        self._graph_for('net', lambda: self._run_ops(self.num_network_ops)).replay()
       else:
-        self._run_ops(net_upto)
+        self._run_ops(self.num_network_ops)
       return
     sidx = self._step % 2
     ring = self._step % 4
@@ -611,17 +591,10 @@ class Engine(LaunchList):
     else:
       if self._nms_pending[sidx]:
         main.wait_event(self._ev_nms[sidx])      # the NMS that last read this buffer set is done
-      def net_and_pre():
-        self._fused_target = self._post[sidx] if self.fuse_class_argmax else None
-        try:
-          self._run_ops(net_upto)
-        finally:
-          self._fused_target = None
-        self._pre_ops[sidx]()
       if self.use_cuda_graph:
-        self._graph_for(('net+pre', sidx), net_and_pre).replay()
+        self._graph_for(('net+pre', sidx), lambda: self._net_and_pre(sidx)).replay()
       else:
-        net_and_pre()
+        self._net_and_pre(sidx)
       self._ev_pre[sidx].record(main)
       self._enqueue_nms(sidx, after_nms, ring)
     self._cur = sidx
@@ -653,82 +626,64 @@ class Engine(LaunchList):
                     small maps) -- runs under the backbone of the NEXT step
       NMS stream  : NMS-V5 (+ after_nms hook)
 
-    The only tensors the two halves share are the backbone features P3..P5.
-    defer_heads=False: the head stage of step i is enqueued right away and overlaps the EARLY
-      backbone of step i+1.  No copy of P3..P5 is needed: the backbone is cut in two graphs at the
-      first launch that writes one of them (blocks_4/project in D0, 1.6 ms into the backbone) and
-      the main stream waits there for the first BiFPN cell of the previous step -- their only
-      reader -- which by then has long finished.
-    defer_heads=True: the head stage of step i is held back until step i+1 has been submitted and
-      starts when its early backbone is done, so that the ~100 short head launches overlap the
-      LATE, small-map backbone layers (blocks_5.. in D0) instead of the bandwidth-bound first
-      layers.  P3..P5 are then copied (35 MB in D0, ~12 us) at the end of the backbone, and the
-      head stage reads the copies.  flush() / wait_detections() submit a held-back head stage."""
-    split, nb, nbc, net_upto = self._bb_split, self.num_backbone_ops, self._heads_start, self.num_network_ops
+    The only tensors the two halves share are the backbone features P3..P5.  The head stage of
+    step i is enqueued right away and overlaps the early backbone of step i+1.  No copy of P3..P5
+    is needed: the backbone is cut in two graphs (bb1, bb2) at the first launch that writes one of
+    them (blocks_4/project in D0, 1.6 ms into the backbone) and the main stream waits there for the
+    first BiFPN cell of the previous step (cell0) -- their only reader -- which by then has long
+    finished."""
+    split, nb = self._bb_split, self.num_backbone_ops
     if self.use_cuda_graph and (self._graph is None or ('heads+pre', sidx) not in self._graph):
       # One eager forward (kernel attributes, module loading), then the captures -- which execute
       # nothing -- so the partial graphs are never run out of order: bb2 alone would add the SE
       # sums of its first block onto a stale accumulator.
       if self._graph is None or 'bb1' not in self._graph:
-        self._run_ops(net_upto)
+        self._run_ops(self.num_network_ops)
         for sx in (0, 1):
           (self._pre_ops_full[sx] if self._pre_ops_full else self._pre_ops[sx])()
     self._replay('bb1', lambda: self._run_ops(split))
-    if self.defer_heads:
-      self._ev_early.record(main)
-      self.flush(after=self._ev_early)          # head + NMS stages of the previous step
-      self._replay('bb2', lambda: self._run_ops(nb, start=split))
-      if self._head_pending:
-        main.wait_event(self._ev_head)          # first BiFPN cell of the previous step read the copies
-      self._replay('featcopy', lambda: self._run_ops(nbc, start=nb))
-      self._ev_bb.record(main)
-      self._deferred = (sidx, after_nms, ring)
-    else:
-      if self._head_pending:
-        main.wait_event(self._ev_head)          # previous step's first BiFPN cell has read P3..P5
-      self._replay('bb2', lambda: self._run_ops(nbc, start=split))
-      self._ev_bb.record(main)
-      self._enqueue_heads(sidx, None)
-      self._enqueue_nms(sidx, after_nms, ring)
+    if self._head_pending:
+      main.wait_event(self._ev_head)          # previous step's first BiFPN cell has read P3..P5
+    self._replay('bb2', lambda: self._run_ops(nb, start=split))
+    self._ev_bb.record(main)
+    self._enqueue_heads(sidx)
+    self._enqueue_nms(sidx, after_nms, ring)
 
-  def _enqueue_heads(self, sidx, after):
-    nbc, net_upto = self._heads_start, self.num_network_ops
-    c0 = self._cell0_end if self._cell0_end is not None else nbc
+  def _enqueue_heads(self, sidx):
+    nb = self.num_backbone_ops
+    c0 = self._cell0_end if self._cell0_end is not None else nb
     hs = self._head_stream
     with torch.cuda.stream(hs):
       hs.wait_event(self._ev_bb)
-      if after is not None:
-        hs.wait_event(after)
       if self._nms_pending[sidx]:
         hs.wait_event(self._ev_nms[sidx])      # the NMS that last read this buffer set is done
-      # first BiFPN cell (+ extra levels): the only reader of P3..P5 (or of their copies)
-      self._replay('cell0', lambda: self._run_ops(c0, start=nbc, priority=self._head_priority),
-                   self._head_capture_stream)
+      # first BiFPN cell (+ extra levels): the only reader of P3..P5
+      self._replay('cell0', lambda: self._run_ops(c0, start=nb), self._head_capture_stream)
       self._ev_head.record(hs)
-      def heads_and_pre():
-        self._fused_target = self._post[sidx] if self.fuse_class_argmax else None
-        try:
-          self._run_ops(net_upto, start=c0, priority=self._head_priority)
-        finally:
-          self._fused_target = None
-        self._pre_ops[sidx]()
-      self._replay(('heads+pre', sidx), heads_and_pre, self._head_capture_stream)
+      self._replay(('heads+pre', sidx), lambda: self._net_and_pre(sidx, start=c0),
+                   self._head_capture_stream)
       self._ev_pre[sidx].record(hs)
     self._head_pending = True
 
-  def flush(self, after=None):
-    """Submits the head + NMS stages of the latest step if they are being held back
-    (defer_heads); `after`: an event they additionally wait for.  No-op otherwise."""
-    if self._deferred is not None:
-      sidx, after_nms, ring = self._deferred
-      self._deferred = None
-      with torch.cuda.device(self.device):
-        self._enqueue_heads(sidx, after)
-        self._enqueue_nms(sidx, after_nms, ring)
+  @contextlib.contextmanager
+  def _class_head_into(self, sidx):
+    """Inside: the fused class head (fuse_class_argmax) writes scores / classes into
+    post-processing set `sidx` instead of logits; sidx None: logits."""
+    self._fused_target = self._post[sidx] if sidx is not None and self.fuse_class_argmax else None
+    try:
+      yield
+    finally:
+      self._fused_target = None
+
+  def _net_and_pre(self, sidx, start=0):
+    """Ops [start, num_network_ops) with the class head writing into post-processing set `sidx`,
+    then that set's pre-NMS."""
+    with self._class_head_into(sidx):
+      self._run_ops(self.num_network_ops, start=start)
+    self._pre_ops[sidx]()
 
   def wait_detections(self):
     """Makes the current stream wait for the NMS (and after_nms hook) of the latest step."""
-    self.flush()
     torch.cuda.current_stream(self.device).wait_event(self._ev_nms[self._cur])
 
   def set_input(self, images):
@@ -777,7 +732,6 @@ class Engine(LaunchList):
       raise ValueError('pre-NMS needs the object_detection head; config.heads = %s'
                        % (self.arch.heads,))
     with torch.cuda.device(self.device):
-      self.flush()
       main = torch.cuda.current_stream(self.device)
       if self._logits_current:
         if self._nms_pending[self._cur]:
@@ -800,13 +754,9 @@ class Engine(LaunchList):
     """Times every launch of the list individually with CUDA events on the current stream
     (eager launches, not the graph) and returns op_info rows extended with 'ms' (mean)."""
     upto = len(self._ops) if postprocess else self.num_network_ops
-    self.flush()
-    if postprocess and self.fuse_class_argmax:
-      self._fused_target = self._post[0]       # time the launches run(postprocess=True) makes
-    try:
+    # postprocess: time the launches run(postprocess=True) makes
+    with self._class_head_into(0 if postprocess else None):
       return self._profile_ops(iters, upto)
-    finally:
-      self._fused_target = None
 
   def _profile_ops(self, iters, upto):
     with torch.cuda.device(self.device):

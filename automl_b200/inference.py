@@ -173,23 +173,18 @@ def _rgb3(v):
 
 class _Request(object):
   """Handle of one in-flight request (ServingDriver.submit, submit_segment, submit_tta): `result()`
-  blocks until the request's results are in its slot's pinned memory and returns `collect(slot)`.
-  `flush` (detection) releases a head / NMS stage the engine may still be holding back."""
+  blocks until the request's results are in its slot's pinned memory and returns `collect(slot)`."""
 
-  def __init__(self, slot, collect, flush=None):
-    self._slot, self._collect, self._flush = slot, collect, flush
+  def __init__(self, slot, collect):
+    self._slot, self._collect = slot, collect
     self._out = None
     slot.pending = self
 
   def done(self):
-    if self._out is None and self._flush is not None:
-      self._flush()
     return self._out is not None or self._slot.ev_done.query()
 
   def result(self):
     if self._out is None:
-      if self._flush is not None:
-        self._flush()
       self._slot.ev_done.synchronize()
       self._out = self._collect(self._slot)
       if self._slot.pending is self:
@@ -391,7 +386,7 @@ class ServingDriver(object):
         slot.ev_done.record(torch.cuda.current_stream())
       eng.run(postprocess=True, after_nms=after_nms)
     # float32 [N (x world), max_output_size, 7]: [image_id, ymin, xmin, ymax, xmax, score, class]
-    return _Request(slot, lambda s: s.host_det.numpy().copy(), flush=eng.flush)
+    return _Request(slot, lambda s: s.host_det.numpy().copy())
 
   def serve_images(self, image_arrays):
     """image_arrays: list (or array) of HxWx3 uint8 images -> float32 [N, max_output_size, 7].

@@ -86,7 +86,7 @@ class LaunchList(object):
 
     Op i then uses the same slot in the eager passes and in every graph that contains it, which
     is safe because one op of one list is never in flight twice: the graphs and eager passes that
-    share ops are ordered on one stream (Engine: net, net+pre, bb1, bb2 and featcopy on the main
+    share ops are ordered on one stream (Engine: net, net+pre, bb1 and bb2 on the main
     stream; cell0 and heads+pre on the head stream, over ops the main-stream stages of the
     pipelined step do not run; forward()
     waits for a pending head stage first), and a side stream of a parallel branch forks from and

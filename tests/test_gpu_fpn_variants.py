@@ -246,7 +246,7 @@ def test_qufpn_pipelined_graph_and_eager_runs_agree(over):
   want = [eager.detect(x).clone() for x in xs]
   graph = _engine(c, w, 2, use_cuda_graph=True, pipeline=False)
   pipe = _engine(c, w, 2, use_cuda_graph=True, pipeline=True)
-  assert pipe._heads_start < pipe._cell0_end < pipe.num_network_ops  # pylint: disable=protected-access
+  assert pipe.num_backbone_ops < pipe._cell0_end < pipe.num_network_ops  # pylint: disable=protected-access
   got = [torch.empty_like(want[0]) for _ in xs]
   for i, x in enumerate(xs):
     pipe.input.copy_(x, non_blocking=True)

@@ -273,15 +273,13 @@ def test_efficientdet_call_surface():
   assert cls_out[3].dtype == torch.float32
 
 
-@pytest.mark.parametrize('defer', [False, True])
 @pytest.mark.parametrize('graph', [True, False])
-def test_pipelined_steps_equal_sequential_steps(graph, defer):
+def test_pipelined_steps_equal_sequential_steps(graph):
   """Engine(pipeline=True) overlaps the backbone of step i+1 with the feature network / heads /
-  pre-NMS of step i and the NMS of step i (three streams, partial graphs; defer_heads=True holds
-  the head stage of a step back until the next step's early backbone is done and reads copies of
-  P3..P5).  Six consecutive steps on six different inputs and image scales, enqueued without any
-  host synchronisation in between, must give bit-identical detections and head outputs to the
-  un-pipelined engine run one step at a time."""
+  pre-NMS of step i and the NMS of step i (three streams, partial graphs).  Six consecutive steps
+  on six different inputs and image scales, enqueued without any host synchronisation in between,
+  must give bit-identical detections and head outputs to the un-pipelined engine run one step at a
+  time."""
   c, a, w, _ = _setup('efficientdet-d0', 128, 2, seed=11)
   rng = np.random.default_rng(12)
   xs = [torch.from_numpy(rng.uniform(-2, 2, size=(2, 128, 128, 3)).astype(np.float32)).cuda() for _ in range(6)]
@@ -293,9 +291,9 @@ def test_pipelined_steps_equal_sequential_steps(graph, defer):
     want_cls.append(seq.box_out[a.levels[0]].clone())   # (the class logits are not stored by detect)
   torch.cuda.synchronize()
   assert not torch.equal(want[0][..., 1:5], want[1][..., 1:5])
-  pipe = _engine(c, w, 2, use_cuda_graph=graph, pipeline=True, defer_heads=defer)
-  assert pipe.pipeline and pipe.defer_heads == defer
-  assert 0 < pipe._bb_split < pipe.num_backbone_ops <= pipe._heads_start < pipe._cell0_end < pipe.num_network_ops  # pylint: disable=protected-access
+  pipe = _engine(c, w, 2, use_cuda_graph=graph, pipeline=True)
+  assert pipe.pipeline
+  assert 0 < pipe._bb_split < pipe.num_backbone_ops < pipe._cell0_end < pipe.num_network_ops  # pylint: disable=protected-access
   got = [torch.empty_like(want[0]) for _ in xs]
   for i, x in enumerate(xs):
     pipe.input.copy_(x, non_blocking=True)     # main stream: ordered after the previous stem
@@ -310,7 +308,7 @@ def test_pipelined_steps_equal_sequential_steps(graph, defer):
   _, box_out = pipe.forward(xs[0])
   torch.cuda.synchronize()
   assert torch.equal(box_out[a.levels[0]], want_cls[0][..., :box_out[a.levels[0]].shape[-1]])
-  # detect() right after (a held-back head stage is flushed by wait_detections)
+  # detect() right after
   assert torch.equal(pipe.detect(xs[2], scales[2]), want[2])
 
 

@@ -366,13 +366,11 @@ def test_binding_is_per_thread(global_slots):
 
 
 # ---- b. one launch list -------------------------------------------------------------------------
-@pytest.mark.parametrize('pipeline,defer_heads', [(False, False), (True, False), (True, True)],
-                         ids=['single_graph', 'pipelined', 'deferred_heads'])
-def test_engine_ops_keep_their_own_slots(pipeline, defer_heads, global_slots):
+@pytest.mark.parametrize('pipeline', [False, True], ids=['single_graph', 'pipelined'])
+def test_engine_ops_keep_their_own_slots(pipeline, global_slots):
   from automl_b200.engine import Engine
   c = _det_config()
-  eng = Engine(c, weights.synthetic_weights(DetArch(c), 0), 2, pipeline=pipeline,
-               defer_heads=defer_heads)
+  eng = Engine(c, weights.synthetic_weights(DetArch(c), 0), 2, pipeline=pipeline)
   rec = Recorder(eng)
   x = _images(1, 2)
   eng.forward(x)
@@ -384,8 +382,6 @@ def test_engine_ops_keep_their_own_slots(pipeline, defer_heads, global_slots):
   rec.check_pool_clean()
   if pipeline:
     want = {'net', 'bb1', 'bb2', 'cell0', ('heads+pre', 0), ('heads+pre', 1)}
-    if defer_heads:
-      want.add('featcopy')
   else:
     want = {'net', ('net+pre', 0), ('net+pre', 1)}
   assert want <= set(eng._graph), sorted(map(str, eng._graph))

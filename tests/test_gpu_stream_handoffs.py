@@ -2,7 +2,7 @@
 stage stalled in turn.
 
 A detection request crosses up to six streams: the driver's copy stream (H2D), the main stream
-(pre-process, bb1, bb2 / featcopy), the engine's head stream (cell0, heads+pre), its NMS stream
+(pre-process, bb1, bb2), the engine's head stream (cell0, heads+pre), its NMS stream
 (NMS, then the after_nms D2H), the driver's D2H stream (masks, TTA) and, in eager mode, the branch
 streams of Engine._run_ops; EffNetV2Model adds copy and D2H streams of its own.  At test sizes every
 stage finishes long before the next request reaches it, so comparing pipelined with sequential
@@ -15,7 +15,7 @@ until X has read them (write after read).
 The stall points are patched in from this file; the product code has no hooks for them:
   h2d            the copy streams (driver, classifier, serve_stream), after their wait_event
   preprocess     ops.preprocess, preprocess_ragged, preprocess_mirrored and cls_preprocess
-  bb1, bb2, featcopy, cell0, heads+pre   Engine._replay, before the stage runs
+  bb1, bb2, cell0, heads+pre   Engine._replay, before the stage runs
   net, net+pre   the graphs Engine._graph_for returns, before replay
   nms            the engine's NMS stream, after its wait_event
   after_nms      parallel.gather_detections, the first call of the driver's after_nms hook
@@ -74,14 +74,9 @@ HANDOFFS = [
     ('engine.py', 'Engine._enqueue_nms', 'self._nms_stream.wait_event(self._ev_pre[sidx])',
      'test_detection_stream', 'test_control_nms_waits_for_pre_nms'),
     ('engine.py', 'Engine._run_pipelined', 'main.wait_event(self._ev_head)', 'test_detection_stream',
-     'test_control_deferred_backbone_waits_for_cell0'),
-    ('engine.py', 'Engine._run_pipelined', 'main.wait_event(self._ev_head)', 'test_detection_stream',
      'test_control_backbone_waits_for_cell0'),
     ('engine.py', 'Engine._enqueue_heads', 'hs.wait_event(self._ev_bb)', 'test_detection_stream',
      'test_control_heads_wait_for_backbone'),
-    ('engine.py', 'Engine._enqueue_heads', 'hs.wait_event(after)', 'test_detection_stream',
-     'no control: it holds the deferred head stage behind the next step\'s early backbone so that '
-     'the two overlap well; no buffer depends on it'),
     ('engine.py', 'Engine._enqueue_heads', 'hs.wait_event(self._ev_nms[sidx])', 'test_detection_stream',
      'test_control_heads_wait_for_nms'),
     ('engine.py', 'Engine.wait_detections',
@@ -335,15 +330,13 @@ def _cached(cache, key, build):
 
 # ---- detection: ServingDriver.serve_stream / submit -----------------------------------------------
 MODES = {   # EDET_* settings the engines are built with, and whether they replay graphs
-    'pipelined': ({'EDET_PIPELINE': '1', 'EDET_DEFER_HEADS': '0'}, True),
-    'deferred': ({'EDET_PIPELINE': '1', 'EDET_DEFER_HEADS': '1'}, True),
-    'sequential': ({'EDET_PIPELINE': '0', 'EDET_DEFER_HEADS': '0'}, True),
-    'eager': ({'EDET_PIPELINE': '1', 'EDET_DEFER_HEADS': '0'}, False),
+    'pipelined': ({'EDET_PIPELINE': '1'}, True),
+    'sequential': ({'EDET_PIPELINE': '0'}, True),
+    'eager': ({'EDET_PIPELINE': '1'}, False),
 }
 PIPELINED = ('h2d', 'preprocess', 'bb1', 'bb2', 'cell0', 'heads+pre', 'nms', 'after_nms')
 DETECTION_POINTS = {
     'pipelined': PIPELINED,
-    'deferred': PIPELINED + ('featcopy',),
     'sequential': ('h2d', 'preprocess', 'net+pre', 'nms', 'after_nms'),
     'eager': PIPELINED + ('branch',),
 }
@@ -747,12 +740,6 @@ def test_control_nms_waits_for_pre_nms(cache):
 
 def test_control_backbone_waits_for_cell0(cache):
   drv, eng, reqs, want = _uniform_stream(cache, 'pipelined')
-  _expect_caught(lambda: _run_stream(drv, reqs, want, ['cell0'], None),
-                 [(torch.cuda.current_stream(), eng._ev_head)])    # pylint: disable=protected-access
-
-
-def test_control_deferred_backbone_waits_for_cell0(cache):
-  drv, eng, reqs, want = _uniform_stream(cache, 'deferred')
   _expect_caught(lambda: _run_stream(drv, reqs, want, ['cell0'], None),
                  [(torch.cuda.current_stream(), eng._ev_head)])    # pylint: disable=protected-access
 
