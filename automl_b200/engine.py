@@ -558,7 +558,7 @@ class Engine(LaunchList):
       self._graph[key] = capture_graph(fn, capture_stream)
     return self._graph[key]
 
-  def run(self, postprocess=True, after_nms=None):
+  def run(self, postprocess=True, after_nms=None, after_heads=None):
     """Enqueues one forward from self.input.
 
     postprocess=False: network only, on the current stream (writes every head output).
@@ -568,10 +568,19 @@ class Engine(LaunchList):
       (pipeline=False: network + pre-NMS as one graph on the current stream, only the NMS overlaps
       the next step).  The class logits are not stored on this path (fuse_class_argmax).  Call
       wait_detections() (or detect()) before reading `self.detections` from the current stream.
+
+      after_heads(seg_out), with the segmentation head only: called right after the step's head
+      stage, on the stream that ran it (the head stream; pipeline=False: the current stream), to
+      enqueue work that reads this step's segmentation logits, e.g. the masks.  The step's NMS and
+      after_nms, and any later reader of the head outputs, are ordered after it; the next step's
+      head stage, which rewrites seg_out, runs after it on the same stream.
     """
     if postprocess and not self.arch.has_detection:
       raise ValueError('post-processing needs the object_detection head; config.heads = %s'
                        % (self.arch.heads,))
+    if after_heads is not None and (self.seg_out is None or not postprocess):
+      raise ValueError('after_heads needs the segmentation head and postprocess=True; '
+                       'config.heads = %s' % (self.arch.heads,))
     if not postprocess:
       self._logits_current = True
       if self._head_pending:   # a pipelined step may still be reading / writing the head buffers
@@ -587,7 +596,7 @@ class Engine(LaunchList):
     self._logits_current = not self.fuse_class_argmax
     main = torch.cuda.current_stream(self.device)
     if self.pipeline:
-      self._run_pipelined(sidx, main, after_nms, ring)
+      self._run_pipelined(sidx, main, after_nms, ring, after_heads)
     else:
       if self._nms_pending[sidx]:
         main.wait_event(self._ev_nms[sidx])      # the NMS that last read this buffer set is done
@@ -595,6 +604,8 @@ class Engine(LaunchList):
         self._graph_for(('net+pre', sidx), lambda: self._net_and_pre(sidx)).replay()
       else:
         self._net_and_pre(sidx)
+      if after_heads is not None:
+        after_heads(self.seg_out)
       self._ev_pre[sidx].record(main)
       self._enqueue_nms(sidx, after_nms, ring)
     self._cur = sidx
@@ -618,7 +629,7 @@ class Engine(LaunchList):
     else:
       fn()
 
-  def _run_pipelined(self, sidx, main, after_nms, ring):
+  def _run_pipelined(self, sidx, main, after_nms, ring, after_heads):
     """One step as three overlapping stages:
 
       main stream : stem + MBConv blocks of THIS step (throughput bound: the large maps)
@@ -646,10 +657,10 @@ class Engine(LaunchList):
       main.wait_event(self._ev_head)          # previous step's first BiFPN cell has read P3..P5
     self._replay('bb2', lambda: self._run_ops(nb, start=split))
     self._ev_bb.record(main)
-    self._enqueue_heads(sidx)
+    self._enqueue_heads(sidx, after_heads)
     self._enqueue_nms(sidx, after_nms, ring)
 
-  def _enqueue_heads(self, sidx):
+  def _enqueue_heads(self, sidx, after_heads):
     nb = self.num_backbone_ops
     c0 = self._cell0_end if self._cell0_end is not None else nb
     hs = self._head_stream
@@ -662,6 +673,8 @@ class Engine(LaunchList):
       self._ev_head.record(hs)
       self._replay(('heads+pre', sidx), lambda: self._net_and_pre(sidx, start=c0),
                    self._head_capture_stream)
+      if after_heads is not None:     # outside the graphs: it changes with every request
+        after_heads(self.seg_out)
       self._ev_pre[sidx].record(hs)
     self._head_pending = True
 

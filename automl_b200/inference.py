@@ -25,6 +25,9 @@ size) or edet_preprocess_ragged (sizes differ; one launch either way) -> network
 -> D2H copy of the [N, max_output_size, 7] detections.  With 'segmentation' in the config's heads,
 segment_images / segment_stream run the same staging and pre-process, the network without NMS,
 then edet_seg_masks -> one D2H copy of a uint8 mask per image at the image's own size.
+serve_images_with_masks / serve_stream_with_masks (both heads) return the detections and the masks
+of the same images from one pipelined pass: edet_seg_masks runs on the engine's head stream right
+after the step's head stage, and the masks are copied to the host behind the detections.
 serve_images_tta / serve_stream_tta (flip test-time augmentation) pre-process each image and its
 mirror in one launch (edet_preprocess_mirrored), run the network on the 2N batch, per-class NMS
 (edet_per_class_nms) over all 2N, then weighted box fusion (edet_wbf) -> one D2H copy of the
@@ -165,6 +168,14 @@ def segment_request(image_arrays, image_size, num_classes):
   return (shapes,) + seg_mask_table(shapes, image_size)
 
 
+def _unpack_masks(packed, shapes):
+  """The uint8 [h, w] numpy masks of images of sizes `shapes` [(h, w), ...] from the pinned buffer
+  `packed`, where they lie back to back as seg_mask_table lays them out."""
+  offsets = np.cumsum([0] + [h * w for h, w in shapes])
+  host = packed[:offsets[-1]].numpy().copy()
+  return [host[o:o + h * w].reshape(h, w) for o, (h, w) in zip(offsets, shapes)]
+
+
 def _rgb3(v):
   if isinstance(v, (int, float)):
     return [float(v)] * 3
@@ -172,8 +183,9 @@ def _rgb3(v):
 
 
 class _Request(object):
-  """Handle of one in-flight request (ServingDriver.submit, submit_segment, submit_tta): `result()`
-  blocks until the request's results are in its slot's pinned memory and returns `collect(slot)`."""
+  """Handle of one in-flight request (ServingDriver.submit, submit_segment, submit_tta,
+  submit_with_masks): `result()` blocks until the request's results are in its slot's pinned memory
+  and returns `collect(slot)`."""
 
   def __init__(self, slot, collect):
     self._slot, self._collect = slot, collect
@@ -228,7 +240,9 @@ class _Slot(object):
                      if world > 1 else None)
     self.masks_dev = self.masks_host = None    # segmentation: the packed uint8 masks
     self.tta = None                            # flip TTA: _TTABuffers
-    self.ev_out = torch.cuda.Event()           # after the request's last kernel (masks, TTA)
+    # before the D2H stream's copy: after the request's last kernel (masks, TTA), or after the
+    # detection copy of a request with masks
+    self.ev_out = torch.cuda.Event()
     self.ev_done = torch.cuda.Event()          # its results are in pinned memory
     self.pending = None                        # its handle, until the results are collected
 
@@ -305,8 +319,11 @@ class ServingDriver(object):
     """Checks one request (staging.decoded_images, against batch_size) and takes the next slot of
     the engine of `views` x N images, building the driver on first use: (the decoded request, the
     engine, the slot).  The slot's previous request is completed first, as its buffers are about to
-    be reused.  Nothing is enqueued."""
-    request = staging.decoded_images(image_arrays, self.batch_size or None, self.device)
+    be reused.  Nothing is enqueued.  A request that is already a staging.Decoded is not checked
+    again."""
+    request = image_arrays
+    if not isinstance(request, staging.Decoded):
+      request = staging.decoded_images(image_arrays, self.batch_size or None, self.device)
     if self._engines is None:
       self.build()
     n = views * len(request.shapes)
@@ -402,6 +419,33 @@ class ServingDriver(object):
     return staging.pipelined(self.submit, batches, self.MAX_IN_FLIGHT)
 
   # ---- segmentation --------------------------------------------------------------------------
+  def _check_masks(self, resize):
+    """The refusals every mask request shares, raised before anything is built or enqueued."""
+    if resize != 'nearest':
+      raise NotImplementedError('mask resize %r: only nearest sampling is built' % (resize,))
+    if torch.distributed.is_available() and torch.distributed.is_initialized():
+      raise NotImplementedError('segmentation masks under torch.distributed are not built')
+
+  def _stage_masks(self, eng, slot, request):
+    """Stages a mask request in the slot with its mask table riding in the same H2D copy (_stage)
+    and grows the slot's mask buffers to its packed masks: (device view of the table, packed byte
+    count).  The slot's previous request has completed (_acquire), so neither buffer is in use."""
+    table, total = seg_mask_table(request.shapes, tuple(eng.input.shape[1:3]))
+    dev_table = self._stage(eng, slot, request, table=table)
+    slot.masks_dev = staging.grow(slot.masks_dev, total, device=self.device)
+    slot.masks_host = staging.grow(slot.masks_host, total, pin_memory=True)
+    return dev_table, total
+
+  def _launch_masks(self, eng, slot, request, num_classes, dev_table):
+    """edet_seg_masks from the engine's segmentation logits into the slot's mask buffer, on the
+    current stream, which then releases the slot's staging: the kernel has read the table."""
+    hs, ws = eng.seg_out.shape[1:3]
+    f = 2 ** (self.config.min_level - 1)
+    assert (hs * f, ws * f) == tuple(eng.input.shape[1:3]), 'logits grid is not input / f'
+    ops.seg_masks(eng.seg_out, num_classes, f, dev_table,
+                  tuple(int(v) for v in np.max(request.shapes, axis=0)), slot.masks_dev)
+    slot.staging.release()
+
   def submit_segment(self, image_arrays, resize='nearest'):
     """Enqueues one segmentation request and returns a handle; `handle.result()` blocks until the
     masks are in host memory: a list of uint8 [h_i, w_i] numpy arrays, the class of every pixel of
@@ -414,36 +458,19 @@ class ServingDriver(object):
     takes the arg-max over the classes (first class on ties, like tf.argmax in the reference's
     segmentation demo).  The packed masks reach pinned host memory in one D2H copy on a stream of
     their own, so up to MAX_IN_FLIGHT requests overlap like detection requests do."""
-    if resize != 'nearest':
-      raise NotImplementedError('mask resize %r: only nearest sampling is built' % (resize,))
-    if torch.distributed.is_available() and torch.distributed.is_initialized():
-      raise NotImplementedError('segmentation masks under torch.distributed are not built')
+    self._check_masks(resize)
     heads = self.params.get('heads') or []
     if 'segmentation' not in heads:
       raise ValueError("segmentation masks need 'segmentation' in heads; heads = %s" % (heads,))
     with torch.cuda.device(self.device):
       request, eng, slot = self._acquire(image_arrays)
       num_classes = _mask_classes(self.config.seg_num_classes)
-      table, total = seg_mask_table(request.shapes, tuple(eng.input.shape[1:3]))
-      dev_table = self._stage(eng, slot, request, table=table)
+      dev_table, total = self._stage_masks(eng, slot, request)
       eng.run(postprocess=False)
-      # the slot's previous request has completed (_acquire), so neither buffer is still in use
-      slot.masks_dev = staging.grow(slot.masks_dev, total, device=self.device)
-      slot.masks_host = staging.grow(slot.masks_host, total, pin_memory=True)
-      hs, ws = eng.seg_out.shape[1:3]
-      f = 2 ** (self.config.min_level - 1)
-      assert (hs * f, ws * f) == tuple(eng.input.shape[1:3]), 'logits grid is not input / f'
-      ops.seg_masks(eng.seg_out, num_classes, f, dev_table,
-                    tuple(int(v) for v in np.max(request.shapes, axis=0)), slot.masks_dev)
-      slot.staging.release()               # the mask kernel has read the table
+      self._launch_masks(eng, slot, request, num_classes, dev_table)
       self._download(slot, slot.masks_dev[:total], slot.masks_host[:total])
     shapes = request.shapes
-
-    def masks(s):
-      packed = s.masks_host[:total].numpy().copy()
-      offsets = np.cumsum([0] + [h * w for h, w in shapes])
-      return [packed[o:o + h * w].reshape(h, w) for o, (h, w) in zip(offsets, shapes)]
-    return _Request(slot, masks)
+    return _Request(slot, lambda s: _unpack_masks(s.masks_host, shapes))
 
   def segment_images(self, image_arrays, resize='nearest'):
     """image_arrays: list of HxWx3 uint8 images (sizes may differ) or a uint8 [N, h, w, 3] tensor
@@ -454,6 +481,58 @@ class ServingDriver(object):
     """Generator over an iterable of requests: yields the masks of each, in order, keeping
     MAX_IN_FLIGHT requests in flight."""
     return staging.pipelined(lambda b: self.submit_segment(b, resize), batches, self.MAX_IN_FLIGHT)
+
+  # ---- detections and masks from one pass ------------------------------------------------------
+  def submit_with_masks(self, image_arrays, resize='nearest'):
+    """Enqueues one request for detections and segmentation masks of the same images and returns a
+    handle; `handle.result()` blocks until both are in host memory and returns (detections, masks):
+    what submit() and submit_segment() return for the request, from one network pass.  Needs a
+    config whose `heads` hold both 'object_detection' and 'segmentation', and at most 256 classes.
+
+    The request is staged as in submit_segment() and runs the pipelined step of submit(): the
+    step's head stage computes the segmentation logits with the class and box outputs, and the
+    edet_seg_masks launch follows it on the engine's head stream (Engine.run's after_heads), so the
+    backbone of the next request still overlaps this one's heads.  The detections are copied to
+    pinned memory on the NMS stream, the masks behind them on the D2H stream.  Combined requests
+    share the slots of every other request kind.  The checks of submit() and submit_segment() are
+    raised before anything is built or enqueued."""
+    self._check_masks(resize)
+    heads = self.params.get('heads') or []
+    if 'object_detection' not in heads or 'segmentation' not in heads:
+      raise ValueError("detections with masks need 'object_detection' and 'segmentation' in heads; "
+                       "heads = %s" % (heads,))
+    num_classes = _mask_classes(self.config.seg_num_classes if self._engines is not None
+                                else self.params['seg_num_classes'])
+    request = staging.decoded_images(image_arrays, self.batch_size or None, self.device)
+    with torch.cuda.device(self.device):
+      request, eng, slot = self._acquire(request)
+      dev_table, total = self._stage_masks(eng, slot, request)
+
+      def after_heads(seg_out, slot=slot):
+        """On the engine's head stream, before the next request's head stage rewrites seg_out: the
+        masks, and the staging release after the one kernel that reads the table."""
+        self._launch_masks(eng, slot, request, num_classes, dev_table)
+
+      def after_nms(det, slot=slot):
+        """On the engine's NMS stream, which waits for the head stage and after_heads: the
+        detections, then the masks on the D2H stream behind that copy (_download records ev_out
+        here), so the slot's ev_done follows both copies."""
+        slot.host_det.copy_(det, non_blocking=True)
+        self._download(slot, slot.masks_dev[:total], slot.masks_host[:total])
+      eng.run(postprocess=True, after_nms=after_nms, after_heads=after_heads)
+    shapes = request.shapes
+    return _Request(slot, lambda s: (s.host_det.numpy().copy(), _unpack_masks(s.masks_host, shapes)))
+
+  def serve_images_with_masks(self, image_arrays):
+    """image_arrays: list of HxWx3 uint8 images (sizes may differ) or a uint8 [N, h, w, 3] tensor
+    -> (float32 [N, max_output_size, 7] detections, list of uint8 [h_i, w_i] masks), see
+    submit_with_masks."""
+    return self.submit_with_masks(image_arrays).result()
+
+  def serve_stream_with_masks(self, batches):
+    """Generator over an iterable of requests: yields (detections, masks) of each, in order,
+    keeping MAX_IN_FLIGHT requests in flight."""
+    return staging.pipelined(self.submit_with_masks, batches, self.MAX_IN_FLIGHT)
 
   # ---- flip test-time augmentation --------------------------------------------------------------
   def submit_tta(self, image_arrays):
